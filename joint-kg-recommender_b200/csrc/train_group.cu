@@ -626,9 +626,9 @@ k_group_step_e(const GroupArgs G, const float up0, const float* __restrict__ up_
 // byte count, so the warp waits once per group and then reads its rows with conflict-free LDS.128 (lane = chunk).
 // The ring is warp-local (the same warp produces and consumes: no CTA barrier, no empty-slot barrier -- program
 // order plus a proxy fence orders the reads of a stage before the bulk copies that refill it), and it keeps
-// (S - 1) x (3 + K) x 400 B per warp in flight without holding a register: 125 KB per SM at 8 warps x 4 stages.
-// The arithmetic and the gradient stores are k_group_step_e's.  Whether this beats register loads + L1 prefetch
-// depends on where the table lives (L2-resident 100k entities vs 500k / 5M), so it is selected only by KGREC_GROUP_STEP.
+// (S - 1) x (3 + K) x 400 B per warp in flight without holding a register.  The arithmetic and the gradient stores
+// are k_group_step_e's.  kgrec_corrupt_loss_step runs it with 16 warps x 2 stages (166 KB of shared memory at
+// d = 100, K = 10) for slot gradients without the fused regulariser; see group_step_tma_smem for the measurement.
 template <bool L1, bool DENSE, bool MARGIN, int W>
 __global__ void __launch_bounds__(W * 32, 1)
 k_group_step_e_tma(const GroupArgs G, const float up0, float* __restrict__ pos_scores, float* __restrict__ neg_scores,
@@ -732,7 +732,10 @@ k_group_step_e_tma(const GroupArgs G, const float up0, float* __restrict__ pos_s
       if (act) x = lds_f4(st_addr + (3 + k) * d4);
       const float4 B = head ? bt : bh;
       const float4 e = make_float4(B.x - x.x, B.y - x.y, B.z - x.z, B.w - x.w);
-      const float sn = warp_sum(dist_term(e.x, L1) + dist_term(e.y, L1) + dist_term(e.z, L1) + dist_term(e.w, L1));
+      // L2: the rounding k_group_step_e's compiled sum has (y*y first, then x, z, w by FMA), so that scores, the hinge
+      // decisions and with them every gradient are the register kernel's bit for bit
+      const float sn = warp_sum(L1 ? fabsf(e.x) + fabsf(e.y) + fabsf(e.z) + fabsf(e.w)
+                                   : __fmaf_rn(e.w, e.w, __fmaf_rn(e.z, e.z, __fmaf_rn(e.x, e.x, __fmul_rn(e.y, e.y)))));
       if (lane == k) mys = sn;
       float coef;
       if (MARGIN) {
@@ -1678,18 +1681,13 @@ static const char* group_step_env() {
   return cached[0] ? cached : nullptr;
 }
 
-// TMA-staged variant of the TransE step kernel: encoded as 16 * warps + stages, 0 = register-load kernel.
-// KGREC_GROUP_STEP=t<w><s> forces it (w: 8 -> 8 warps, c -> 12, g -> 16; s = stages 2..6), anything else the default.
-static int group_step_tma_mode(const kgrec_tables* T, int n_neg, int reg_flags) {
-  const char* env = group_step_env();
-  if (reg_flags) return 0;
-  if (env && env[0] == 't' && env[1] && env[2]) {
-    const int W = env[1] == '8' ? 8 : (env[1] == 'c' ? 12 : 16), S = env[2] - '0';
-    if (S < 2 || S > 6) return 0;
-    const size_t smem = static_cast<size_t>(W) * S * (136 + static_cast<size_t>(3 + n_neg) * T->dim * 4) + 128;
-    return smem <= 225 * 1024 ? 16 * W + S : 0;
-  }
-  return 0;
+// The TMA-staged TransE step kernel runs 16 warps per CTA with 2 stages per warp; it is picked for slot gradients when
+// that ring fits one CTA's shared memory.  On an H100 (400 W) at bench.py's shape (d = 100, K = 10, 262 144 groups) it
+// took 0.91 / 1.03 / 1.07 ms per launch against 1.00 / 1.22 / 1.30 ms for the register kernel at |E| = 100k / 500k / 5M.
+constexpr int kTmaWarps = 16, kTmaStages = 2;
+static size_t group_step_tma_smem(int dim, int n_neg) {
+  return ((static_cast<size_t>(kTmaWarps) * kTmaStages * (8 + 128) + 127) & ~static_cast<size_t>(127)) +
+         static_cast<size_t>(kTmaWarps) * kTmaStages * (3 + n_neg) * dim * 4;
 }
 
 static int group_check(const kgrec_tables* T, int model, Plan* pl, const void* ph, const void* pt, const void* pr,
@@ -1920,24 +1918,26 @@ extern "C" int kgrec_corrupt_loss_step(const kgrec_tables* tables, int model, co
   const char* env = group_step_env();
   const bool small32 = n_neg <= 32 && static_cast<double>(n_pos) * (2 + n_neg) * tables->dim * 4 < 4.0e9 &&
                        static_cast<double>(n_pos) * n_neg < 2.0e9;          // 32-bit slot offsets, scores kept in lanes
-  const int tma_mode = group_step_tma_mode(tables, n_neg, reg_flags);   // TMA-staged gather (A/B switch or the size rule)
-  if (pl.fam == FAM_E && pl.nch == 1 && small32 && tma_mode && n_neg <= 29 && tables->ld == tables->dim) {
-    const int W = tma_mode / 16, S = tma_mode % 16;
-    const size_t smem = ((static_cast<size_t>(W) * S * (8 + 128) + 127) & ~static_cast<size_t>(127)) +
-                        static_cast<size_t>(W) * S * (3 + n_neg) * tables->dim * 4;
-    int64_t ctas = (n_pos + W - 1) / W;
+  // slot gradients of TransE at d <= 128 without the fused regulariser: the TMA-staged gather when its ring fits and
+  // every warp gets at least two groups (with one, the second stage has nothing to overlap and a single 1024-positive
+  // batch runs faster on the register kernel); KGREC_GROUP_STEP = 0 / n / 3 keep the general or register kernels
+  const bool tma = pl.fam == FAM_E && pl.nch == 1 && small32 && grads->mode == 0 && !reg_flags && n_neg <= 29 &&
+                   tables->ld == tables->dim && !(env && (env[0] == '0' || env[0] == 'n' || env[0] == '3')) &&
+                   group_step_tma_smem(tables->dim, n_neg) <= 225 * 1024 &&
+                   n_pos >= static_cast<int64_t>(kTmaStages) * kTmaWarps * sm_count();
+  if (tma) {
+    const size_t smem = group_step_tma_smem(tables->dim, n_neg);
+    int64_t ctas = (n_pos + kTmaWarps - 1) / kTmaWarps;
     if (ctas > sm_count()) ctas = sm_count();
-#define CALL_T(L1V, DV, MV, WV)                                                                                         \
+#define CALL_T(L1V, MV)                                                                                                 \
   {                                                                                                                     \
-    auto kern = k_group_step_e_tma<L1V, DV, MV, WV>;                                                                    \
+    auto kern = k_group_step_e_tma<L1V, false, MV, kTmaWarps>;                                                          \
     KGREC_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));      \
-    kern<<<static_cast<int>(ctas), WV * 32, smem, st>>>(G, grad_loss, pos_scores, neg_scores, group_loss, *grads, slot_ent_ids, slot_rel_ids, status, S); \
+    kern<<<static_cast<int>(ctas), kTmaWarps * 32, smem, st>>>(G, grad_loss, pos_scores, neg_scores, group_loss, *grads, slot_ent_ids, slot_rel_ids, status, kTmaStages); \
   }
-#define CALL_TW(L1V, DV, MV) { if (W == 8) CALL_T(L1V, DV, MV, 8) else if (W == 12) CALL_T(L1V, DV, MV, 12) else CALL_T(L1V, DV, MV, 16) }
-    const bool dn = grads->mode == 1, mg = loss_kind == KGREC_LOSS_MARGIN;
-    if (tables->l1) { if (dn) { if (mg) CALL_TW(true, true, true) else CALL_TW(true, true, false) } else { if (mg) CALL_TW(true, false, true) else CALL_TW(true, false, false) } }
-    else { if (dn) { if (mg) CALL_TW(false, true, true) else CALL_TW(false, true, false) } else { if (mg) CALL_TW(false, false, true) else CALL_TW(false, false, false) } }
-#undef CALL_TW
+    const bool mg = loss_kind == KGREC_LOSS_MARGIN;
+    if (tables->l1) { if (mg) CALL_T(true, true) else CALL_T(true, false) }
+    else { if (mg) CALL_T(false, true) else CALL_T(false, false) }
 #undef CALL_T
   } else if (pl.fam == FAM_E && pl.nch == 1 && small32 && !(env && env[0] == '0')) {
 #define CALL_E(L1V, DV, MV)                                                                                      \
