@@ -65,6 +65,30 @@ __device__ __forceinline__ float warp_reduce_scatter8(float (&v)[8], int lane) {
   return r;
 }
 
+// Reduce-scatter of N (16 or 32) per-lane partials with xor offsets 16, 8, 4, 2, 1, warp_sum's order: every sum is
+// formed by warp_sum's pairing tree, so it is warp_sum(v[i]) bit for bit.  N = 32: lane l returns the sum of v[l]
+// (31 shuffles); N = 16: lanes 2i and 2i + 1 return the sum of v[i] (16 shuffles).
+template <int N>
+__device__ __forceinline__ float warp_reduce_scatter(float (&v)[N], int lane) {
+  static_assert(N == 16 || N == 32, "16 or 32 partials");
+#pragma unroll
+  for (int l = 0; l < (N == 32 ? 5 : 4); ++l) {
+    const int o = 16 >> l, n = N >> (l + 1);
+    const bool up = (lane & o) != 0;          // this lane keeps the upper half of the remaining sums
+#pragma unroll
+    for (int i = 0; i < N / 2; ++i) {
+      if (i < n) {
+        const float send = up ? v[i] : v[i + n];
+        const float keep = up ? v[i + n] : v[i];
+        v[i] = keep + __shfl_xor_sync(FULL, send, o);
+      }
+    }
+  }
+  float r = v[0];
+  if (N == 16) r += __shfl_xor_sync(FULL, r, 1);
+  return r;
+}
+
 // ---- index loads --------------------------------------------------------------
 __device__ __forceinline__ int64_t load_idx(const void* p, int64_t i, int is64) {
   return is64 ? __ldg(reinterpret_cast<const long long*>(p) + i)
@@ -122,6 +146,13 @@ __device__ __forceinline__ void bulk_g2s(void* dst, const void* src, uint32_t by
   asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(
                    smem_u32(dst)),
                "l"(src), "r"(bytes), "r"(smem_u32(bar))
+               : "memory");
+}
+// the same copy with an L2 cache policy on its global reads (see policy_evict_last)
+__device__ __forceinline__ void bulk_g2s_hint(void* dst, const void* src, uint32_t bytes, uint64_t* bar, uint64_t pol) {
+  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1], %2, [%3], %4;" ::"r"(
+                   smem_u32(dst)),
+               "l"(src), "r"(bytes), "r"(smem_u32(bar)), "l"(pol)
                : "memory");
 }
 

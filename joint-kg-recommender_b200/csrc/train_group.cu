@@ -625,15 +625,31 @@ k_group_step_e(const GroupArgs G, const float up0, const float* __restrict__ up_
 // lane that holds its id, into the warp's own ring of S stages; a stage carries an mbarrier armed with the group's
 // byte count, so the warp waits once per group and then reads its rows with conflict-free LDS.128 (lane = chunk).
 // The ring is warp-local (the same warp produces and consumes: no CTA barrier, no empty-slot barrier -- program
-// order plus a proxy fence orders the reads of a stage before the bulk copies that refill it), and it keeps
-// (S - 1) x (3 + K) x 400 B per warp in flight without holding a register.  The arithmetic and the gradient stores
-// are k_group_step_e's.  kgrec_corrupt_loss_step runs it with 16 warps x 2 stages (166 KB of shared memory at
-// d = 100, K = 10) for slot gradients without the fused regulariser; see group_step_tma_smem for the measurement.
-template <bool L1, bool DENSE, bool MARGIN, int W>
+// order plus a proxy fence orders the reads of a stage before the bulk copies that refill it).  The copies read the
+// tables with the evict_last policy on the share G.keep of their lines, as k_group_step_e's loads do; the gradient
+// stores are evict_first.  What bounds the kernel is one warp's serial path through a group, so that path is short:
+//   * ids ahead: the ids of the group a stage takes next are loaded into registers one group before its copies are
+//     issued, so neither the id ring nor the copy addresses wait on a global round trip;
+//   * load first, release early: all 3 + K rows of a group (one float4 per lane each) are read before any
+//     arithmetic, and the stage is refilled with the group S ahead right away -- the proxy fence waits on those
+//     LDS, not on the previous group's stores, and the refill overlaps this group's arithmetic;
+//   * one reduction: the per-lane partials of the 1 + K distances go through one reduce-scatter (xor 16 .. 1, the
+//     pairing tree of warp_sum, so every score is warp_sum's bit for bit) instead of 1 + K dependent trees;
+//   * coefficients in parallel: the hinge / BPR terms of all negatives are computed at once in their lanes and
+//     handed to the gradient pass by broadcast; lsum, cpos and the shared-row accumulators are summed in k order,
+//     so scores, losses and every gradient slot are those of k_group_step_e bit for bit.
+// NS = 16 (K <= 15) keeps the rows of a group in registers.  With NS = 32 (16 <= K <= 29) they do not fit: the rows
+// are read once for the scores and again for the gradients, and the stage is released after the second read.
+// kgrec_corrupt_loss_step runs it with kTmaWarps x kTmaStages for slot gradients without the fused regulariser; see
+// group_step_tma_smem for the measurement.
+template <bool L1, bool MARGIN, int W, int NS>
 __global__ void __launch_bounds__(W * 32, 1)
 k_group_step_e_tma(const GroupArgs G, const float up0, float* __restrict__ pos_scores, float* __restrict__ neg_scores,
                    float* __restrict__ group_loss, const kgrec_grads Gr, int64_t* __restrict__ slot_ent,
                    int64_t* __restrict__ slot_rel, int32_t* status, const int S) {
+  static_assert(NS == 16 || NS == 32, "a group's scores are reduced over 16 or 32 slots");
+  constexpr int NK = NS - 1;        // most negatives: their partials in slots 0 .. K-1, the positive's in slot NS - 1
+  constexpr bool KEEP = NS == 16;   // every row of a group stays in registers
   extern __shared__ __align__(128) unsigned char smem_raw[];
   const kgrec_tables& T = G.T;
   const LossCfg& L = G.L;
@@ -643,7 +659,7 @@ k_group_step_e_tma(const GroupArgs G, const float up0, float* __restrict__ pos_s
   const uint32_t n_ent = static_cast<uint32_t>(T.n_ent);
   const uint32_t ld4 = static_cast<uint32_t>(T.ld) * 4u, d4 = static_cast<uint32_t>(T.dim) * 4u;
   const int bp = static_cast<int>(L.batch_pos < 0x7fffffff ? L.batch_pos : 0x7fffffff);
-  const uint64_t pol_stream = policy_evict_first();
+  const uint64_t pol_keep = policy_evict_last(G.keep), pol_stream = policy_evict_first();
   const bool act = lane * 4 < T.dim;
   // shared-memory map: [W][S] mbarriers | [W][S][32] int32 compact ids | [W][S][n_rows] rows of d4 bytes
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem_raw) + wid * S;
@@ -663,16 +679,20 @@ k_group_step_e_tma(const GroupArgs G, const float up0, float* __restrict__ pos_s
   bool bad = false;
   const void* pcol = lane == 0 ? G.ph : (lane == 1 ? G.pt : G.pr);
 
-  // producer half: ids of group jj -> ring slot, one bulk copy per row
-  auto issue = [&](int jj, int s) {
-    // lane 0..2: h, t, r of the positive; lane 3..3+K-1: corrupted entity of negative lane-3 (sign = head replaced)
+  // ids of group jj as loaded, one per lane: 0..2 h, t, r of the positive; 3..3+K-1 corrupted entity of negative
+  // lane-3 (sign = head replaced).  Nothing uses them before the next call of issue().
+  auto fetch = [&](int jj) -> int64_t {
+    if (lane < 3) return load_idx(pcol, jj, G.is64);
+    return lane < n_rows ? static_cast<int64_t>(__ldg(G.corrupt + static_cast<uint32_t>(jj) * K + (lane - 3))) : 0;
+  };
+  // producer half: checked ids -> ring slot, one bulk copy per row
+  auto issue = [&](int64_t pv, int s) {
     int32_t v = 0;
     if (lane < 3) {
-      const int64_t pv = load_idx(pcol, jj, G.is64);
       const int64_t lim = lane == 2 ? T.n_rel : T.n_ent;
       if (static_cast<uint64_t>(pv) >= static_cast<uint64_t>(lim)) bad = true; else v = static_cast<int32_t>(pv);
     } else if (lane < n_rows) {
-      v = __ldg(G.corrupt + static_cast<uint32_t>(jj) * K + (lane - 3));
+      v = static_cast<int32_t>(pv);
       const uint32_t id = static_cast<uint32_t>(v < 0 ? ~v : v);
       if (id >= n_ent) { bad = true; v = 0; }
     }
@@ -682,93 +702,132 @@ k_group_step_e_tma(const GroupArgs G, const float up0, float* __restrict__ pos_s
     if (lane < n_rows) {
       const uint32_t id = lane < 3 ? static_cast<uint32_t>(v) : static_cast<uint32_t>(v < 0 ? ~v : v);
       const char* src = reinterpret_cast<const char*>(lane == 2 ? T.rel : T.ent) + static_cast<uint64_t>(id) * ld4;
-      bulk_g2s(rows_base + static_cast<size_t>(s) * stage_bytes + static_cast<size_t>(lane) * d4, src, d4, bars + s);
+      bulk_g2s_hint(rows_base + static_cast<size_t>(s) * stage_bytes + static_cast<size_t>(lane) * d4, src, d4, bars + s,
+                    pol_keep);
     }
+  };
+  auto sub4 = [](const float4& a, const float4& b) { return make_float4(a.x - b.x, a.y - b.y, a.z - b.z, a.w - b.w); };
+  // L2: the rounding k_group_step_e's compiled sum has (y*y first, then x, z, w by FMA), so that scores, the hinge
+  // decisions and with them every gradient are the register kernel's bit for bit
+  auto dist4 = [](const float4& e) {
+    return L1 ? fabsf(e.x) + fabsf(e.y) + fabsf(e.z) + fabsf(e.w)
+              : __fmaf_rn(e.w, e.w, __fmaf_rn(e.z, e.z, __fmaf_rn(e.x, e.x, __fmul_rn(e.y, e.y))));
   };
 
   int j = blockIdx.x * W + wid;
-  for (int s = 0, jj = j; s < S - 1 && jj < n_pos; ++s, jj += stride) issue(jj, s);
+  for (int s = 0, jj = j; s < S && jj < n_pos; ++s, jj += stride) issue(fetch(jj), s);
+  int64_t nv = j + S * stride < n_pos ? fetch(j + S * stride) : 0;      // ids of the next group to issue
   for (int it = 0; j < n_pos; j += stride, ++it) {
     const int s = it % S;
-    {   // keep S - 1 groups in flight: refill the stage consumed in the previous iteration
-      const int jn = j + (S - 1) * stride;
-      if (jn < n_pos) {
-        fence_proxy_async_smem();
-        __syncwarp();
-        issue(jn, (it + S - 1) % S);
-      }
-    }
     mbar_wait(bars + s, static_cast<uint32_t>(it / S) & 1u);
     const int32_t myid = ids_ring[s * 32 + lane];
     const uint32_t st_addr = smem_u32(rows_base + static_cast<size_t>(s) * stage_bytes) + lane * 16;
-    const uint32_t ih0 = static_cast<uint32_t>(__shfl_sync(FULL, myid, 0)), it0 = static_cast<uint32_t>(__shfl_sync(FULL, myid, 1)),
-                   ir0 = static_cast<uint32_t>(__shfl_sync(FULL, myid, 2));
+    auto release = [&]() {      // refill this stage with the group S ahead, and fetch the ids of the one after it
+      const int jr = j + S * stride;
+      if (jr < n_pos) {
+        fence_proxy_async_smem();
+        __syncwarp();
+        issue(nv, s);
+        if (jr + stride < n_pos) nv = fetch(jr + stride);
+      }
+    };
+    float4 h = z4, t = z4, r = z4;
+    float4 x[KEEP ? NK : 1];    // KEEP: the corrupted rows, then their residuals
+    if (act) { h = lds_f4(st_addr); t = lds_f4(st_addr + d4); r = lds_f4(st_addr + 2 * d4); }
+    if (KEEP) {
+#pragma unroll
+      for (int k = 0; k < NK; ++k) {
+        x[k] = z4;
+        if (k < K && act) x[k] = lds_f4(st_addr + (3 + k) * d4);
+      }
+      release();
+    }
+    const uint32_t hm = __ballot_sync(FULL, myid < 0) >> 3;      // bit k: negative k replaced the head
     if (slot_ent) {
       const uint32_t s0 = static_cast<uint32_t>(j) * (2 + K);
       if (lane < 2) slot_ent[s0 + lane] = myid;
       if (lane == 2) slot_rel[j] = myid;
       if (lane >= 3 && lane < n_rows) slot_ent[s0 + lane - 1] = myid < 0 ? ~myid : myid;
     }
-    float4 h = z4, t = z4, r = z4;
-    if (act) { h = lds_f4(st_addr); t = lds_f4(st_addr + d4); r = lds_f4(st_addr + 2 * d4); }
+    const float4 bh = make_float4(h.x + r.x, h.y + r.y, h.z + r.z, h.w + r.w);
+    const float4 bt = make_float4(t.x - r.x, t.y - r.y, t.z - r.z, t.w - r.w);
+    const float4 ep = sub4(bh, t);
+    // the residual of negative k: e' = B - x with B = h + r (tail replaced) or t - r (head replaced)
+    auto residual = [&](int k) {
+      float4 xk = z4;
+      if (KEEP) xk = x[k];
+      else if (act) xk = lds_f4(st_addr + (3 + k) * d4);
+      return sub4((hm >> k) & 1u ? bt : bh, xk);
+    };
+    float p[NS];
+#pragma unroll
+    for (int k = 0; k < NS; ++k) p[k] = 0.f;
+    p[NS - 1] = dist4(ep);
+#pragma unroll
+    for (int k = 0; k < NK; ++k) {
+      if (k < K) {
+        const float4 e = residual(k);
+        if (KEEP) x[k] = e;
+        p[k] = dist4(e);
+      }
+    }
+    const float sv = warp_reduce_scatter<NS>(p, lane);       // score of slot (NS == 32 ? lane : lane / 2)
+    const float sp = __shfl_sync(FULL, sv, 31);
+    const int kl = NS == 32 ? lane : lane >> 1;
+    const bool mine = kl < K && (NS == 32 || (lane & 1) == 0);   // this lane holds negative kl's score
+    if (mine) neg_scores[static_cast<uint32_t>(j) * K + kl] = sv;
     float up = up0;
     if (!MARGIN) {
       const int b = j / bp;
       up /= static_cast<float>(min(bp, n_pos - b * bp)) * static_cast<float>(K);
     }
-    const float4 bh = make_float4(h.x + r.x, h.y + r.y, h.z + r.z, h.w + r.w);
-    const float4 bt = make_float4(t.x - r.x, t.y - r.y, t.z - r.z, t.w - r.w);
-    const float4 ep = make_float4(bh.x - t.x, bh.y - t.y, bh.z - t.z, bh.w - t.w);
-    const float sp = warp_sum(dist_term(ep.x, L1) + dist_term(ep.y, L1) + dist_term(ep.z, L1) + dist_term(ep.w, L1));
-    float lsum = 0.f, cpos = 0.f, mys = 0.f;
+    // every negative's loss term and coefficient at once, in its lane
+    float lt, dq = 0.f;
+    uint32_t am = 0;                // MARGIN: bit (lane of k) set when negative k's hinge is active
+    if (MARGIN) {
+      const float tt = sp - sv + prm;
+      lt = fmaxf(tt, 0.f);
+      am = __ballot_sync(FULL, mine && tt > 0.f);
+    } else {
+      const float xx = prm * (sp - sv);
+      lt = fmaxf(-xx, 0.f) + log1pf(expf(-fabsf(xx)));
+      dq = -prm / (1.f + expf(xx));
+    }
+    float lsum = 0.f, cpos = MARGIN ? static_cast<float>(__popc(am)) : 0.f;   // a sum of ones is exact in any order
     float4 accT = z4, accH = z4;
     uint32_t goff = (static_cast<uint32_t>(j) * (2 + K) + 2) * d4;
-#pragma unroll 2
-    for (int k = 0; k < K; ++k) {
-      const int32_t c = __shfl_sync(FULL, myid, 3 + k);
-      const bool head = c < 0;
-      const uint32_t id = static_cast<uint32_t>(head ? ~c : c);
-      float4 x = z4;
-      if (act) x = lds_f4(st_addr + (3 + k) * d4);
-      const float4 B = head ? bt : bh;
-      const float4 e = make_float4(B.x - x.x, B.y - x.y, B.z - x.z, B.w - x.w);
-      // L2: the rounding k_group_step_e's compiled sum has (y*y first, then x, z, w by FMA), so that scores, the hinge
-      // decisions and with them every gradient are the register kernel's bit for bit
-      const float sn = warp_sum(L1 ? fabsf(e.x) + fabsf(e.y) + fabsf(e.z) + fabsf(e.w)
-                                   : __fmaf_rn(e.w, e.w, __fmaf_rn(e.z, e.z, __fmaf_rn(e.x, e.x, __fmul_rn(e.y, e.y)))));
-      if (lane == k) mys = sn;
-      float coef;
-      if (MARGIN) {
-        const float tt = sp - sn + prm;
-        lsum += fmaxf(tt, 0.f);
-        coef = tt > 0.f ? up : 0.f;
-        cpos += tt > 0.f ? 1.f : 0.f;
-      } else {
-        const float xx = prm * (sp - sn);
-        lsum += fmaxf(-xx, 0.f) + log1pf(expf(-fabsf(xx)));
-        const float dp = -prm / (1.f + expf(xx));
-        cpos += dp;
-        coef = dp * up;
-      }
-      if (coef != 0.f) {
-        float4 gc;
-        if (L1) {
-          gc = make_float4(coef * ddist_term(e.x, 1), coef * ddist_term(e.y, 1), coef * ddist_term(e.z, 1), coef * ddist_term(e.w, 1));
+#pragma unroll
+    for (int k = 0; k < NK; ++k) {
+      if (k < K) {
+        constexpr int kw = NS == 32 ? 1 : 2;
+        lsum += __shfl_sync(FULL, lt, kw * k);
+        float coef;                 // -(dLoss/dsn): the corrupted row's gradient is coef * dL(e')/de'
+        if (MARGIN) {
+          coef = (am >> (kw * k)) & 1u ? up : 0.f;
         } else {
-          const float c2 = 2.f * coef;
-          gc = make_float4(c2 * e.x, c2 * e.y, c2 * e.z, c2 * e.w);
+          const float dp = __shfl_sync(FULL, dq, kw * k);
+          cpos += dp;
+          coef = dp * up;
         }
-        if (head) { accH.x -= gc.x; accH.y -= gc.y; accH.z -= gc.z; accH.w -= gc.w; }
-        else { accT.x -= gc.x; accT.y -= gc.y; accT.z -= gc.z; accT.w -= gc.w; }
-        if (act) {
-          if (DENSE) red_add_f4(reinterpret_cast<float*>(gent_b + static_cast<uint64_t>(id) * d4), gc.x, gc.y, gc.z, gc.w);
-          else stg_f4_hint(reinterpret_cast<float4*>(gent_b + goff), gc.x, gc.y, gc.z, gc.w, pol_stream);
+        if (coef != 0.f) {          // warp-uniform: an inactive hinge has no gradient
+          const float4 e = KEEP ? x[k] : residual(k);     // KEEP: x holds the residuals now
+          float4 gc;
+          if (L1) {
+            gc = make_float4(coef * ddist_term(e.x, 1), coef * ddist_term(e.y, 1), coef * ddist_term(e.z, 1), coef * ddist_term(e.w, 1));
+          } else {
+            const float c2 = 2.f * coef;
+            gc = make_float4(c2 * e.x, c2 * e.y, c2 * e.z, c2 * e.w);
+          }
+          if ((hm >> k) & 1u) { accH.x -= gc.x; accH.y -= gc.y; accH.z -= gc.z; accH.w -= gc.w; }
+          else { accT.x -= gc.x; accT.y -= gc.y; accT.z -= gc.z; accT.w -= gc.w; }
+          if (act) stg_f4_hint(reinterpret_cast<float4*>(gent_b + goff), gc.x, gc.y, gc.z, gc.w, pol_stream);
+        } else if (act) {
+          stg_f4_hint(reinterpret_cast<float4*>(gent_b + goff), 0.f, 0.f, 0.f, 0.f, pol_stream);
         }
-      } else if (!DENSE) {
-        if (act) stg_f4_hint(reinterpret_cast<float4*>(gent_b + goff), 0.f, 0.f, 0.f, 0.f, pol_stream);
+        goff += d4;
       }
-      goff += d4;
     }
+    if (!KEEP) release();
     const float cp = cpos * up;
     const float4 eps = make_float4(cp * ddist_term(ep.x, L1), cp * ddist_term(ep.y, L1), cp * ddist_term(ep.z, L1), cp * ddist_term(ep.w, L1));
     const float4 gh = make_float4(accT.x + eps.x, accT.y + eps.y, accT.z + eps.z, accT.w + eps.w);
@@ -778,18 +837,11 @@ k_group_step_e_tma(const GroupArgs G, const float up0, float* __restrict__ pos_s
       pos_scores[j] = sp;
       group_loss[j] = lsum;
     }
-    if (lane < K) neg_scores[static_cast<uint32_t>(j) * K + lane] = mys;
     if (act) {
-      if (DENSE) {
-        red_add_f4(reinterpret_cast<float*>(gent_b + static_cast<uint64_t>(ih0) * d4), gh.x, gh.y, gh.z, gh.w);
-        red_add_f4(reinterpret_cast<float*>(gent_b + static_cast<uint64_t>(it0) * d4), gt.x, gt.y, gt.z, gt.w);
-        red_add_f4(reinterpret_cast<float*>(grel_b + static_cast<uint64_t>(ir0) * d4), gr.x, gr.y, gr.z, gr.w);
-      } else {
-        const uint32_t g0 = static_cast<uint32_t>(j) * (2 + K) * d4;
-        stg_f4_hint(reinterpret_cast<float4*>(gent_b + g0), gh.x, gh.y, gh.z, gh.w, pol_stream);
-        stg_f4_hint(reinterpret_cast<float4*>(gent_b + g0 + d4), gt.x, gt.y, gt.z, gt.w, pol_stream);
-        stg_f4_hint(reinterpret_cast<float4*>(grel_b + static_cast<uint32_t>(j) * d4), gr.x, gr.y, gr.z, gr.w, pol_stream);
-      }
+      const uint32_t g0 = static_cast<uint32_t>(j) * (2 + K) * d4;
+      stg_f4_hint(reinterpret_cast<float4*>(gent_b + g0), gh.x, gh.y, gh.z, gh.w, pol_stream);
+      stg_f4_hint(reinterpret_cast<float4*>(gent_b + g0 + d4), gt.x, gt.y, gt.z, gt.w, pol_stream);
+      stg_f4_hint(reinterpret_cast<float4*>(grel_b + static_cast<uint32_t>(j) * d4), gr.x, gr.y, gr.z, gr.w, pol_stream);
     }
   }
   if (bad && status) *status = 1;
@@ -1682,8 +1734,10 @@ static const char* group_step_env() {
 }
 
 // The TMA-staged TransE step kernel runs 16 warps per CTA with 2 stages per warp; it is picked for slot gradients when
-// that ring fits one CTA's shared memory.  On an H100 (400 W) at bench.py's shape (d = 100, K = 10, 262 144 groups) it
-// took 0.91 / 1.03 / 1.07 ms per launch against 1.00 / 1.22 / 1.30 ms for the register kernel at |E| = 100k / 500k / 5M.
+// that ring fits one CTA's shared memory.  Warps x stages measured with the current loop on an H100 80GB HBM3 (400 W)
+// at bench.py's shape (d = 100, K = 10, 262 144 groups), ms per launch at |E| = 10k / 100k (tools/step_e_floor.py):
+//   16 x 2: 0.77 / 0.89    14 x 3: 0.78 / 0.93    12 x 3: 0.82 / 1.00
+//   20 x 2: 0.79 / 1.09, and it spills (20 warps leave 96 registers a thread; the 16-slot loop needs ~114)
 constexpr int kTmaWarps = 16, kTmaStages = 2;
 static size_t group_step_tma_smem(int dim, int n_neg) {
   return ((static_cast<size_t>(kTmaWarps) * kTmaStages * (8 + 128) + 127) & ~static_cast<size_t>(127)) +
@@ -1929,15 +1983,17 @@ extern "C" int kgrec_corrupt_loss_step(const kgrec_tables* tables, int model, co
     const size_t smem = group_step_tma_smem(tables->dim, n_neg);
     int64_t ctas = (n_pos + kTmaWarps - 1) / kTmaWarps;
     if (ctas > sm_count()) ctas = sm_count();
-#define CALL_T(L1V, MV)                                                                                                 \
+#define CALL_T(L1V, MV, NSV)                                                                                            \
   {                                                                                                                     \
-    auto kern = k_group_step_e_tma<L1V, false, MV, kTmaWarps>;                                                          \
+    auto kern = k_group_step_e_tma<L1V, MV, kTmaWarps, NSV>;                                                            \
     KGREC_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));      \
     kern<<<static_cast<int>(ctas), kTmaWarps * 32, smem, st>>>(G, grad_loss, pos_scores, neg_scores, group_loss, *grads, slot_ent_ids, slot_rel_ids, status, kTmaStages); \
   }
+#define CALL_TN(L1V, MV) { if (n_neg < 16) CALL_T(L1V, MV, 16) else CALL_T(L1V, MV, 32) }
     const bool mg = loss_kind == KGREC_LOSS_MARGIN;
-    if (tables->l1) { if (mg) CALL_T(true, true) else CALL_T(true, false) }
-    else { if (mg) CALL_T(false, true) else CALL_T(false, false) }
+    if (tables->l1) { if (mg) CALL_TN(true, true) else CALL_TN(true, false) }
+    else { if (mg) CALL_TN(false, true) else CALL_TN(false, false) }
+#undef CALL_TN
 #undef CALL_T
   } else if (pl.fam == FAM_E && pl.nch == 1 && small32 && !(env && env[0] == '0')) {
 #define CALL_E(L1V, DV, MV)                                                                                      \
