@@ -337,6 +337,67 @@ int kgrec_rec_rows_step(const kgrec_tables* tables, int model, const void* pu, c
                         void* loss_workspace, float* norm_reg_loss, const float* gumbel_u, uint64_t seed,
                         int32_t* status, kgrec_stream_t stream);
 
+/* ---- device-resident step state: training steps replayed from a CUDA graph -----------------------
+ * A replayed graph re-uses every by-value argument it was captured with.  The scalars that change from
+ * one training step to the next therefore live in device memory, in one kgrec_step_state, and the
+ * `_dev` entry points below read them there instead of taking them by value.  Everything else about a
+ * `_dev` call (validation, kernels, results) is that of the entry point it is named after.
+ * A step runs:  kgrec_batch_gather  ->  kgrec_step_advance  ->  samplers / loss step / optimizer (_dev),
+ * so inside a step `step` is the running step's 1-based count and `epoch` its mark epoch. */
+typedef struct kgrec_step_state {
+  int64_t step;          /* steps begun so far: Adam's step count t                               */
+  uint64_t gumbel_seed;  /* Gumbel-noise seed of step s: gumbel_seed + s                          */
+  uint64_t sample_seed;  /* negative-sampler seed of step s: sample_seed + s                      */
+  int32_t epoch;         /* epoch mark of the running step (kgrec_rows_mark / _sqnorm / _update)  */
+  float lr;              /* learning rate of kgrec_rows_update_dev                                */
+} kgrec_step_state;
+
+/* step += 1, epoch += 1, and *cursor += batch when cursor is not NULL (one thread). */
+int kgrec_step_advance(kgrec_step_state* state, int64_t* cursor, int64_t batch, kgrec_stream_t stream);
+/* out_host[c][j] = cols_host[c][order[*cursor + j]] for j < batch, c < n_cols (<= 4): the batch
+ * DeviceTrainIterator cuts from its shuffled visiting order.  The cursor is only read: the
+ * kgrec_step_advance that follows moves it (a kernel cannot read and move it without a grid barrier).
+ * Positions past n_order and rows outside [0, n_rows) read row 0 and set *status (optional) to 1. */
+int kgrec_batch_gather(const int64_t* order, int64_t n_order, const int64_t* cursor, const void* const* cols_host,
+                       void* const* out_host, int n_cols, int idx_bytes, int64_t n_rows, int64_t batch,
+                       int32_t* status, kgrec_stream_t stream);
+/* kgrec_rows_mark / _sqnorm / _update with the epoch, the learning rate and Adam's step (bias terms
+ * formed on the device) read from *state */
+int kgrec_rows_mark_dev(const kgrec_mark_seg* segs_host, int n_segs, const kgrec_step_state* state, int32_t* status,
+                        kgrec_stream_t stream);
+int kgrec_rows_sqnorm_dev(const kgrec_opt_table* tabs_host, int n_tabs, const kgrec_step_state* state, float* sqnorm,
+                          kgrec_stream_t stream);
+int kgrec_rows_update_dev(const kgrec_opt_table* tabs_host, int n_tabs, const kgrec_step_state* state, int kind,
+                          float eps, float beta1, float beta2, float weight_decay, const float* sqnorm,
+                          float max_norm, kgrec_stream_t stream);
+/* the samplers with seed = state->sample_seed + state->step */
+int kgrec_sample_corrupt_dev(const void* ph, const void* pt, const void* pr, int idx_bytes, int64_t n_pos,
+                             int32_t n_neg, int64_t n_ent, int64_t n_rel, const uint64_t* table, int64_t capacity,
+                             const kgrec_step_state* state, int32_t* corrupt, int32_t* status, kgrec_stream_t stream);
+int kgrec_sample_neg_items_dev(const void* u, const void* pi, int idx_bytes, int64_t n, int32_t n_neg, int64_t n_item,
+                               const uint64_t* table, int64_t capacity, const kgrec_step_state* state,
+                               int32_t* neg_items, int32_t* status, kgrec_stream_t stream);
+/* kgrec_rank_loss_step / kgrec_rec_rows_step with the Gumbel seed state->gumbel_seed + state->step
+ * (read only when tables->use_gumbel and gumbel_u is NULL) and, for the row-factored step, the epoch
+ * mark state->epoch */
+int kgrec_rank_loss_step_dev(const kgrec_tables* tables, int model,
+                             const void* pa, const void* pb, const void* pc,
+                             const void* na, const void* nb, const void* nc,
+                             int idx_bytes, int64_t n_pos, int32_t n_neg, int64_t batch_pos,
+                             int loss_kind, float margin_or_target, float grad_loss,
+                             const float* gumbel_u, const kgrec_step_state* state,
+                             float* pos_scores, float* neg_scores, float* loss,
+                             const kgrec_grads* grads,
+                             int64_t* slot_user_ids, int64_t* slot_item_ids, int64_t* slot_ent_ids,
+                             void* workspace, int32_t* status, kgrec_stream_t stream);
+int kgrec_rec_rows_step_dev(const kgrec_tables* tables, int model, const void* pu, const void* pi, const void* ni,
+                            int idx_bytes, int64_t n_pos, int32_t n_neg, int64_t batch_pos, int loss_kind,
+                            float margin_or_target, float grad_loss, const int32_t* marks_user,
+                            const int32_t* marks_item, const kgrec_step_state* state, float* workspace,
+                            int32_t first_use, const kgrec_grads* acc, float* pos_scores, float* neg_scores,
+                            float* loss, void* loss_workspace, float* norm_reg_loss, const float* gumbel_u,
+                            int32_t* status, kgrec_stream_t stream);
+
 /* ---- the drivers' recommendation-side regularisers (utils/loss.py:18-23) -------------------------
  * item_recommendation.py:177-180: normLoss(user rows) + normLoss(item rows of cat[pos, neg]) +
  * normLoss(pref table) + orthogonalLoss(pref, pref_norm); knowledgable_recommendation.py:343-344:

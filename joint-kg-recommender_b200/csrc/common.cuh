@@ -380,4 +380,16 @@ __device__ __forceinline__ float gumbel_fast(uint32_t bits) {
   return -__logf(-__logf(u));
 }
 
+// The Gumbel seed of a training kernel: the by-value argument, or -- for the `_dev` entry points, whose launches are
+// replayed from a CUDA graph -- the running step's seed read from the device step state.  Converts from uint64_t, so
+// the by-value callers are unchanged.
+struct SeedRef {
+  uint64_t value;
+  const kgrec_step_state* state;
+  __host__ __device__ SeedRef(uint64_t v = 0, const kgrec_step_state* s = nullptr) : value(v), state(s) {}
+  __device__ __forceinline__ uint64_t get() const {
+    return state ? state->gumbel_seed + static_cast<uint64_t>(state->step) : value;
+  }
+};
+
 }  // namespace kgrec

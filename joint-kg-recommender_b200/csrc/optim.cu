@@ -27,12 +27,14 @@ struct MarkArgs {
   int64_t begin[kMaxMarkSegs + 1];      // prefix sums of seg[].n
   int n_segs;
   int32_t epoch;
+  const kgrec_step_state* state;        // _dev entry point: the epoch is read here
 };
 
 // marks[id] = epoch for every id of every segment.  compact: the group-compact corrupted-id format
 // (v < 0 names entity ~v).  remap: ids are looked up first (KTUP: item -> aligned entity row).
 __global__ void __launch_bounds__(256) k_rows_mark(const MarkArgs A, int32_t* status) {
   const int64_t total = A.begin[A.n_segs];
+  const int32_t epoch = A.state ? A.state->epoch : A.epoch;
   for (int64_t i = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x; i < total;
        i += static_cast<int64_t>(gridDim.x) * blockDim.x) {
     int s = 0;
@@ -48,7 +50,7 @@ __global__ void __launch_bounds__(256) k_rows_mark(const MarkArgs A, int32_t* st
       v = __ldg(S.remap + v);
     }
     if (static_cast<uint64_t>(v) >= static_cast<uint64_t>(S.rows)) { if (status) *status = 1; v = 0; }
-    S.marks[v] = A.epoch;
+    S.marks[v] = epoch;
   }
 }
 
@@ -62,7 +64,11 @@ struct SweepArgs {
   float lr, eps, beta1, beta2, wd, bias1, bias2_sqrt;
   const float* sqnorm;
   float max_norm;
+  const kgrec_step_state* state;             // _dev entry points: epoch, lr and Adam's step are read here
 };
+
+// The scalars of one step: the by-value arguments, or the device step state's
+__device__ __forceinline__ int32_t sweep_epoch(const SweepArgs& A) { return A.state ? A.state->epoch : A.epoch; }
 
 // A warp owns 32 consecutive rows of one table: one coalesced load of their marks, a ballot, and the marked rows are
 // handed out kRowsInFlight at a time -- f gets the batch so that it can issue the loads of all its rows before the
@@ -70,7 +76,7 @@ struct SweepArgs {
 constexpr int kRowsInFlight = 4;
 
 template <typename F>
-__device__ __forceinline__ void sweep_rows(const SweepArgs& A, F&& f) {
+__device__ __forceinline__ void sweep_rows(const SweepArgs& A, int32_t epoch, F&& f) {
   const int lane = threadIdx.x & 31;
   const int64_t warp = (static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x) >> 5;
   const int64_t n_warps = (static_cast<int64_t>(gridDim.x) * blockDim.x) >> 5;
@@ -83,7 +89,7 @@ __device__ __forceinline__ void sweep_rows(const SweepArgs& A, F&& f) {
     const int64_t row0 = (c - A.chunk_begin[t]) * 32;
     const int64_t row = row0 + lane;
     bool mine = row < T.rows;
-    if (mine && T.marks) mine = __ldg(T.marks + row / A.div[t]) == A.epoch;
+    if (mine && T.marks) mine = __ldg(T.marks + row / A.div[t]) == epoch;
     unsigned m = __ballot_sync(FULL, mine);
     while (m) {
       int64_t rows[kRowsInFlight];
@@ -100,7 +106,7 @@ __device__ __forceinline__ void sweep_rows(const SweepArgs& A, F&& f) {
 
 __global__ void __launch_bounds__(256) k_rows_sqnorm(const SweepArgs A, float* out) {
   float local = 0.f;
-  sweep_rows(A, [&](const kgrec_opt_table& T, const int64_t (&rows)[kRowsInFlight], int n, int lane) {
+  sweep_rows(A, sweep_epoch(A), [&](const kgrec_opt_table& T, const int64_t (&rows)[kRowsInFlight], int n, int lane) {
     const int nch = (T.dim + 3) >> 2;
     for (int ch = lane; ch < nch; ch += 32) {
       if (T.vec) {
@@ -129,25 +135,34 @@ __global__ void __launch_bounds__(256) k_rows_sqnorm(const SweepArgs A, float* o
   }
 }
 
-__device__ __forceinline__ float opt_elem(const SweepArgs& A, float pv, float gv, float* s1, float* s2) {
+struct StepScalars { float lr, bias1, bias2_sqrt; };
+
+__device__ __forceinline__ float opt_elem(const SweepArgs& A, const StepScalars& S, float pv, float gv, float* s1, float* s2) {
   if (A.wd != 0.f) gv = fmaf(A.wd, pv, gv);          // weight_decay = l2_lambda, on touched rows only
-  if (A.kind == OPT_SGD) return pv - A.lr * gv;
+  if (A.kind == OPT_SGD) return pv - S.lr * gv;
   if (A.kind == OPT_ADAGRAD) {                        // torch.optim.Adagrad: sum += g^2 ; p -= lr g / (sqrt(sum) + eps)
     const float s = fmaf(gv, gv, *s1);
     *s1 = s;
-    return pv - A.lr * gv / (sqrtf(s) + A.eps);
+    return pv - S.lr * gv / (sqrtf(s) + A.eps);
   }
   const float m = A.beta1 * *s1 + (1.f - A.beta1) * gv;          // torch.optim.Adam on the touched rows ("lazy")
   const float v = A.beta2 * *s2 + (1.f - A.beta2) * gv * gv;
   *s1 = m;
   *s2 = v;
-  return pv - (A.lr / A.bias1) * m / (sqrtf(v) / A.bias2_sqrt + A.eps);
+  return pv - (S.lr / S.bias1) * m / (sqrtf(v) / S.bias2_sqrt + A.eps);
 }
 
 __global__ void __launch_bounds__(256) k_rows_update(const SweepArgs A) {
   float scale = 1.f;
   if (A.sqnorm) scale = fminf(1.f, A.max_norm / (sqrtf(__ldg(A.sqnorm)) + 1e-6f));   // clip_grad_norm's coefficient
-  sweep_rows(A, [&](const kgrec_opt_table& T, const int64_t (&rows)[kRowsInFlight], int n, int lane) {
+  StepScalars S{A.lr, A.bias1, A.bias2_sqrt};
+  if (A.state) {          // the host formulas of kgrec_rows_update, on the device
+    const float t = static_cast<float>(A.state->step);
+    S.lr = A.state->lr;
+    S.bias1 = 1.f - powf(A.beta1, t);
+    S.bias2_sqrt = sqrtf(1.f - powf(A.beta2, t));
+  }
+  sweep_rows(A, sweep_epoch(A), [&](const kgrec_opt_table& T, const int64_t (&rows)[kRowsInFlight], int n, int lane) {
     const int nch = (T.dim + 3) >> 2;
     const float4 z4 = make_float4(0.f, 0.f, 0.f, 0.f);
     for (int ch = lane; ch < nch; ch += 32) {
@@ -168,10 +183,10 @@ __global__ void __launch_bounds__(256) k_rows_update(const SweepArgs A) {
         for (int i = 0; i < kRowsInFlight; ++i) {
           if (i >= n) continue;
           const int64_t o = rows[i] * T.dim + ch * 4;
-          p[i].x = opt_elem(A, p[i].x, g[i].x * scale, &a[i].x, &b[i].x);
-          p[i].y = opt_elem(A, p[i].y, g[i].y * scale, &a[i].y, &b[i].y);
-          p[i].z = opt_elem(A, p[i].z, g[i].z * scale, &a[i].z, &b[i].z);
-          p[i].w = opt_elem(A, p[i].w, g[i].w * scale, &a[i].w, &b[i].w);
+          p[i].x = opt_elem(A, S, p[i].x, g[i].x * scale, &a[i].x, &b[i].x);
+          p[i].y = opt_elem(A, S, p[i].y, g[i].y * scale, &a[i].y, &b[i].y);
+          p[i].z = opt_elem(A, S, p[i].z, g[i].z * scale, &a[i].z, &b[i].z);
+          p[i].w = opt_elem(A, S, p[i].w, g[i].w * scale, &a[i].w, &b[i].w);
           if (!T.keep_acc) *reinterpret_cast<float4*>(T.acc + o) = z4;                   // zero again after the step
           *reinterpret_cast<float4*>(T.table + o) = p[i];
           if (A.kind != OPT_SGD) *reinterpret_cast<float4*>(T.state1 + o) = a[i];
@@ -184,7 +199,7 @@ __global__ void __launch_bounds__(256) k_rows_update(const SweepArgs A) {
             const float g = T.acc[o];
             if (!T.keep_acc) T.acc[o] = 0.f;
             float a = A.kind != OPT_SGD ? T.state1[o] : 0.f, b = A.kind == OPT_ADAM ? T.state2[o] : 0.f;
-            T.table[o] = opt_elem(A, T.table[o], g * scale, &a, &b);
+            T.table[o] = opt_elem(A, S, T.table[o], g * scale, &a, &b);
             if (A.kind != OPT_SGD) T.state1[o] = a;
             if (A.kind == OPT_ADAM) T.state2[o] = b;
           }
@@ -233,8 +248,8 @@ static int sweep_grid(const SweepArgs& A) {
   return static_cast<int>(ctas < 1 ? 1 : (ctas < cap ? ctas : cap));
 }
 
-extern "C" int kgrec_rows_mark(const kgrec_mark_seg* segs, int n_segs, int32_t epoch, int32_t* status,
-                               kgrec_stream_t stream) {
+static int rows_mark(const kgrec_mark_seg* segs, int n_segs, int32_t epoch, const kgrec_step_state* state,
+                     int32_t* status, kgrec_stream_t stream) {
   if (!segs || n_segs < 1 || n_segs > kMaxMarkSegs) {
     set_error("kgrec_rows_mark: 1..%d id segments per call", kMaxMarkSegs);
     return KGREC_ERR_INVALID;
@@ -242,6 +257,7 @@ extern "C" int kgrec_rows_mark(const kgrec_mark_seg* segs, int n_segs, int32_t e
   MarkArgs A{};
   A.n_segs = n_segs;
   A.epoch = epoch;
+  A.state = state;
   for (int s = 0; s < n_segs; ++s) {
     const kgrec_mark_seg& S = segs[s];
     if (S.n < 0 || (S.n > 0 && (!S.ids || !S.marks)) || (S.idx_bytes != 4 && S.idx_bytes != 8) || S.rows <= 0) {
@@ -260,20 +276,21 @@ extern "C" int kgrec_rows_mark(const kgrec_mark_seg* segs, int n_segs, int32_t e
   return KGREC_OK;
 }
 
-extern "C" int kgrec_rows_sqnorm(const kgrec_opt_table* tabs, int n_tabs, int32_t epoch, float* sqnorm,
-                                 kgrec_stream_t stream) {
+static int rows_sqnorm(const kgrec_opt_table* tabs, int n_tabs, int32_t epoch, const kgrec_step_state* state, float* sqnorm,
+                       kgrec_stream_t stream) {
   SweepArgs A;
   int rc = sweep_args(tabs, n_tabs, epoch, 0, A);
   if (rc) return rc;
+  A.state = state;
   if (!sqnorm) { set_error("sqnorm is NULL"); return KGREC_ERR_INVALID; }
   k_rows_sqnorm<<<sweep_grid(A), 256, 0, static_cast<cudaStream_t>(stream)>>>(A, sqnorm);
   KGREC_CUDA_OK(cudaGetLastError());
   return KGREC_OK;
 }
 
-extern "C" int kgrec_rows_update(const kgrec_opt_table* tabs, int n_tabs, int32_t epoch, int kind, float lr, float eps,
-                                 float beta1, float beta2, int64_t step, float weight_decay, const float* sqnorm,
-                                 float max_norm, kgrec_stream_t stream) {
+static int rows_update(const kgrec_opt_table* tabs, int n_tabs, int32_t epoch, const kgrec_step_state* state, int kind,
+                       float lr, float eps, float beta1, float beta2, int64_t step, float weight_decay,
+                       const float* sqnorm, float max_norm, kgrec_stream_t stream) {
   SweepArgs A;
   int rc = sweep_args(tabs, n_tabs, epoch, 1, A);
   if (rc) return rc;
@@ -286,8 +303,43 @@ extern "C" int kgrec_rows_update(const kgrec_opt_table* tabs, int n_tabs, int32_
   A.kind = kind; A.lr = lr; A.eps = eps; A.beta1 = beta1; A.beta2 = beta2; A.wd = weight_decay;
   A.bias1 = 1.f - powf(beta1, static_cast<float>(step));
   A.bias2_sqrt = sqrtf(1.f - powf(beta2, static_cast<float>(step)));
-  A.sqnorm = sqnorm; A.max_norm = max_norm;
+  A.sqnorm = sqnorm; A.max_norm = max_norm; A.state = state;
   k_rows_update<<<sweep_grid(A), 256, 0, static_cast<cudaStream_t>(stream)>>>(A);
   KGREC_CUDA_OK(cudaGetLastError());
   return KGREC_OK;
+}
+
+extern "C" int kgrec_rows_mark(const kgrec_mark_seg* segs, int n_segs, int32_t epoch, int32_t* status,
+                               kgrec_stream_t stream) {
+  return rows_mark(segs, n_segs, epoch, nullptr, status, stream);
+}
+
+extern "C" int kgrec_rows_sqnorm(const kgrec_opt_table* tabs, int n_tabs, int32_t epoch, float* sqnorm,
+                                 kgrec_stream_t stream) {
+  return rows_sqnorm(tabs, n_tabs, epoch, nullptr, sqnorm, stream);
+}
+
+extern "C" int kgrec_rows_update(const kgrec_opt_table* tabs, int n_tabs, int32_t epoch, int kind, float lr, float eps,
+                                 float beta1, float beta2, int64_t step, float weight_decay, const float* sqnorm,
+                                 float max_norm, kgrec_stream_t stream) {
+  return rows_update(tabs, n_tabs, epoch, nullptr, kind, lr, eps, beta1, beta2, step, weight_decay, sqnorm, max_norm, stream);
+}
+
+extern "C" int kgrec_rows_mark_dev(const kgrec_mark_seg* segs, int n_segs, const kgrec_step_state* state, int32_t* status,
+                                   kgrec_stream_t stream) {
+  if (!state) { set_error("kgrec_rows_mark_dev: step state is NULL"); return KGREC_ERR_INVALID; }
+  return rows_mark(segs, n_segs, 0, state, status, stream);
+}
+
+extern "C" int kgrec_rows_sqnorm_dev(const kgrec_opt_table* tabs, int n_tabs, const kgrec_step_state* state, float* sqnorm,
+                                     kgrec_stream_t stream) {
+  if (!state) { set_error("sparse row optimizer: step state is NULL"); return KGREC_ERR_INVALID; }
+  return rows_sqnorm(tabs, n_tabs, 0, state, sqnorm, stream);
+}
+
+extern "C" int kgrec_rows_update_dev(const kgrec_opt_table* tabs, int n_tabs, const kgrec_step_state* state, int kind,
+                                     float eps, float beta1, float beta2, float weight_decay, const float* sqnorm,
+                                     float max_norm, kgrec_stream_t stream) {
+  if (!state) { set_error("sparse row optimizer: step state is NULL"); return KGREC_ERR_INVALID; }
+  return rows_update(tabs, n_tabs, 0, state, kind, 0.f, eps, beta1, beta2, 1, weight_decay, sqnorm, max_norm, stream);
 }

@@ -60,17 +60,23 @@ struct SampleArgs {
   uint64_t seed;
   int32_t* out;
   int32_t* status;           // optional: set to 2 when a key has no valid negative at all
+  const kgrec_step_state* state;   // _dev entry points: seed = state->sample_seed + state->step
 };
+
+__device__ __forceinline__ uint64_t sample_seed(const SampleArgs& A) {
+  return A.state ? A.state->sample_seed + static_cast<uint64_t>(A.state->step) : A.seed;
+}
 
 constexpr int kMaxAttempts = 64;
 
 __global__ void __launch_bounds__(256) k_sample_corrupt(const SampleArgs A) {
   const int64_t total = A.n_pos * A.n_neg;
+  const uint64_t seed = sample_seed(A);
   for (int64_t m = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x; m < total; m += static_cast<int64_t>(gridDim.x) * blockDim.x) {
     const int64_t j = m / A.n_neg;
     const uint64_t h = static_cast<uint64_t>(load_idx(A.a, j, A.is64)), t = static_cast<uint64_t>(load_idx(A.b, j, A.is64));
     const uint64_t r = static_cast<uint64_t>(load_idx(A.c, j, A.is64));
-    const bool head = philox_uniform_bits(A.seed, static_cast<uint64_t>(m), 0xffffffffu) & 1u;      // random.random() < 0.5
+    const bool head = philox_uniform_bits(seed, static_cast<uint64_t>(m), 0xffffffffu) & 1u;      // random.random() < 0.5
     uint32_t ent = 0;
     auto valid = [&](uint32_t e) {
       if (e == (head ? h : t)) return false;
@@ -82,7 +88,7 @@ __global__ void __launch_bounds__(256) k_sample_corrupt(const SampleArgs A) {
     };
     bool found = false;
     for (int attempt = 0; attempt < kMaxAttempts && !found; ++attempt) {
-      const uint32_t bits = philox_uniform_bits(A.seed, static_cast<uint64_t>(m), static_cast<uint32_t>(attempt));
+      const uint32_t bits = philox_uniform_bits(seed, static_cast<uint64_t>(m), static_cast<uint32_t>(attempt));
       ent = static_cast<uint32_t>((static_cast<uint64_t>(bits) * static_cast<uint64_t>(A.n_cat)) >> 32);   // randrange(entityTotal)
       found = valid(ent);
     }
@@ -100,6 +106,7 @@ __global__ void __launch_bounds__(256) k_sample_corrupt(const SampleArgs A) {
 
 __global__ void __launch_bounds__(256) k_sample_items(const SampleArgs A) {
   const int64_t total = A.n_pos * A.n_neg;
+  const uint64_t seed = sample_seed(A);
   for (int64_t m = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x; m < total; m += static_cast<int64_t>(gridDim.x) * blockDim.x) {
     const int64_t j = m / A.n_neg;
     const uint64_t u = static_cast<uint64_t>(load_idx(A.a, j, A.is64)), pi = static_cast<uint64_t>(load_idx(A.b, j, A.is64));
@@ -109,7 +116,7 @@ __global__ void __launch_bounds__(256) k_sample_items(const SampleArgs A) {
     };
     bool found = false;
     for (int attempt = 0; attempt < kMaxAttempts && !found; ++attempt) {
-      const uint32_t bits = philox_uniform_bits(A.seed, static_cast<uint64_t>(m), static_cast<uint32_t>(attempt));
+      const uint32_t bits = philox_uniform_bits(seed, static_cast<uint64_t>(m), static_cast<uint32_t>(attempt));
       it = static_cast<uint32_t>((static_cast<uint64_t>(bits) * static_cast<uint64_t>(A.n_cat)) >> 32);
       found = valid(it);
     }
@@ -159,27 +166,55 @@ static int sample_check(const void* a, const void* b, int idx_bytes, int64_t n_p
   return KGREC_OK;
 }
 
-extern "C" int kgrec_sample_corrupt(const void* ph, const void* pt, const void* pr, int idx_bytes, int64_t n_pos,
-                                    int32_t n_neg, int64_t n_ent, int64_t n_rel, const uint64_t* table,
-                                    int64_t capacity, uint64_t seed, int32_t* corrupt, int32_t* status, kgrec_stream_t stream) {
+static int sample_corrupt(const void* ph, const void* pt, const void* pr, int idx_bytes, int64_t n_pos, int32_t n_neg,
+                          int64_t n_ent, int64_t n_rel, const uint64_t* table, int64_t capacity, uint64_t seed,
+                          const kgrec_step_state* state, int32_t* corrupt, int32_t* status, kgrec_stream_t stream) {
   int rc = sample_check(ph, pt, idx_bytes, n_pos, n_neg, n_ent, table, capacity, corrupt);
   if (rc) return rc;
   if (!pr || n_rel < 1) { set_error("negative sampler: relations missing"); return KGREC_ERR_INVALID; }
   if (n_pos == 0) return KGREC_OK;
-  const SampleArgs A{ph, pt, pr, idx_bytes == 8, n_pos, n_neg, n_ent, n_rel, table, table ? static_cast<uint64_t>(capacity - 1) : 0, seed, corrupt, status};
+  const SampleArgs A{ph, pt, pr, idx_bytes == 8, n_pos, n_neg, n_ent, n_rel, table, table ? static_cast<uint64_t>(capacity - 1) : 0, seed, corrupt, status, state};
   k_sample_corrupt<<<grid1d(n_pos * n_neg), 256, 0, static_cast<cudaStream_t>(stream)>>>(A);
   KGREC_CUDA_OK(cudaGetLastError());
   return KGREC_OK;
 }
 
-extern "C" int kgrec_sample_neg_items(const void* u, const void* pi, int idx_bytes, int64_t n, int32_t n_neg, int64_t n_item,
-                                      const uint64_t* table, int64_t capacity, uint64_t seed, int32_t* neg_items,
-                                      int32_t* status, kgrec_stream_t stream) {
+static int sample_neg_items(const void* u, const void* pi, int idx_bytes, int64_t n, int32_t n_neg, int64_t n_item,
+                            const uint64_t* table, int64_t capacity, uint64_t seed, const kgrec_step_state* state,
+                            int32_t* neg_items, int32_t* status, kgrec_stream_t stream) {
   int rc = sample_check(u, pi, idx_bytes, n, n_neg, n_item, table, capacity, neg_items);
   if (rc) return rc;
   if (n == 0) return KGREC_OK;
-  const SampleArgs A{u, pi, nullptr, idx_bytes == 8, n, n_neg, n_item, 1, table, table ? static_cast<uint64_t>(capacity - 1) : 0, seed, neg_items, status};
+  const SampleArgs A{u, pi, nullptr, idx_bytes == 8, n, n_neg, n_item, 1, table, table ? static_cast<uint64_t>(capacity - 1) : 0, seed, neg_items, status, state};
   k_sample_items<<<grid1d(n * n_neg), 256, 0, static_cast<cudaStream_t>(stream)>>>(A);
   KGREC_CUDA_OK(cudaGetLastError());
   return KGREC_OK;
+}
+
+extern "C" int kgrec_sample_corrupt(const void* ph, const void* pt, const void* pr, int idx_bytes, int64_t n_pos,
+                                    int32_t n_neg, int64_t n_ent, int64_t n_rel, const uint64_t* table,
+                                    int64_t capacity, uint64_t seed, int32_t* corrupt, int32_t* status, kgrec_stream_t stream) {
+  return sample_corrupt(ph, pt, pr, idx_bytes, n_pos, n_neg, n_ent, n_rel, table, capacity, seed, nullptr, corrupt, status, stream);
+}
+
+extern "C" int kgrec_sample_neg_items(const void* u, const void* pi, int idx_bytes, int64_t n, int32_t n_neg, int64_t n_item,
+                                      const uint64_t* table, int64_t capacity, uint64_t seed, int32_t* neg_items,
+                                      int32_t* status, kgrec_stream_t stream) {
+  return sample_neg_items(u, pi, idx_bytes, n, n_neg, n_item, table, capacity, seed, nullptr, neg_items, status, stream);
+}
+
+extern "C" int kgrec_sample_corrupt_dev(const void* ph, const void* pt, const void* pr, int idx_bytes, int64_t n_pos,
+                                        int32_t n_neg, int64_t n_ent, int64_t n_rel, const uint64_t* table,
+                                        int64_t capacity, const kgrec_step_state* state, int32_t* corrupt, int32_t* status,
+                                        kgrec_stream_t stream) {
+  if (!state) { set_error("negative sampler: step state is NULL"); return KGREC_ERR_INVALID; }
+  return sample_corrupt(ph, pt, pr, idx_bytes, n_pos, n_neg, n_ent, n_rel, table, capacity, 0, state, corrupt, status, stream);
+}
+
+extern "C" int kgrec_sample_neg_items_dev(const void* u, const void* pi, int idx_bytes, int64_t n, int32_t n_neg,
+                                          int64_t n_item, const uint64_t* table, int64_t capacity,
+                                          const kgrec_step_state* state, int32_t* neg_items, int32_t* status,
+                                          kgrec_stream_t stream) {
+  if (!state) { set_error("negative sampler: step state is NULL"); return KGREC_ERR_INVALID; }
+  return sample_neg_items(u, pi, idx_bytes, n, n_neg, n_item, table, capacity, 0, state, neg_items, status, stream);
 }

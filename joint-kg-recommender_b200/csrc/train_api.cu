@@ -5,11 +5,11 @@ namespace kgrec {
 
 #define KGREC_DECLARE_FAMILY(FAMV)                                                                                       \
   extern template int launch_score_fwd<FAMV>(const kgrec_tables&, const Plan&, const IdxArgs&, int64_t, const float*,   \
-                                             uint64_t, float*, int32_t*, cudaStream_t);                                 \
+                                             SeedRef, float*, int32_t*, cudaStream_t);                                 \
   extern template int launch_rank_loss_fwd<FAMV>(const kgrec_tables&, const Plan&, const IdxArgs&, const LossCfg&,      \
-                                                 const float*, uint64_t, float*, float*, float*, int32_t*, cudaStream_t); \
+                                                 const float*, SeedRef, float*, float*, float*, int32_t*, cudaStream_t); \
   extern template int launch_score_bwd<FAMV>(const kgrec_tables&, const Plan&, const IdxArgs&, int64_t, const LossCfg&, \
-                                             const float*, uint64_t, const BwdArgs&, const kgrec_grads&, cudaStream_t);
+                                             const float*, SeedRef, const BwdArgs&, const kgrec_grads&, cudaStream_t);
 KGREC_DECLARE_FAMILY(FAM_E)
 KGREC_DECLARE_FAMILY(FAM_H)
 KGREC_DECLARE_FAMILY(FAM_R)
@@ -183,13 +183,12 @@ extern "C" int kgrec_rank_loss_bwd(const kgrec_tables* tables, int model, const 
                                                    gumbel_u, seed, B, *grads, static_cast<cudaStream_t>(stream));
 }
 
-extern "C" int kgrec_rank_loss_step(const kgrec_tables* tables, int model, const void* pa, const void* pb,
-                                    const void* pc, const void* na, const void* nb, const void* nc, int idx_bytes,
-                                    int64_t n_pos, int32_t n_neg, int64_t batch_pos, int loss_kind,
-                                    float margin_or_target, float grad_loss, const float* gumbel_u, uint64_t seed,
-                                    float* pos_scores, float* neg_scores, float* loss, const kgrec_grads* grads,
-                                    int64_t* slot_user_ids, int64_t* slot_item_ids, int64_t* slot_ent_ids,
-                                    void* workspace, int32_t* status, kgrec_stream_t stream) {
+static int rank_loss_step(const kgrec_tables* tables, int model, const void* pa, const void* pb, const void* pc,
+                          const void* na, const void* nb, const void* nc, int idx_bytes, int64_t n_pos, int32_t n_neg,
+                          int64_t batch_pos, int loss_kind, float margin_or_target, float grad_loss,
+                          const float* gumbel_u, SeedRef seed, float* pos_scores, float* neg_scores, float* loss,
+                          const kgrec_grads* grads, int64_t* slot_user_ids, int64_t* slot_item_ids,
+                          int64_t* slot_ent_ids, void* workspace, int32_t* status, kgrec_stream_t stream) {
   Plan pl;
   int rc = make_plan(tables, model, &pl);
   if (rc) return rc;
@@ -229,4 +228,30 @@ extern "C" int kgrec_rank_loss_step(const kgrec_tables* tables, int model, const
   k_batch_loss<<<static_cast<unsigned>(n_batches), 256, 0, st>>>(group_loss, L, loss);
   KGREC_CUDA_OK(cudaGetLastError());
   return KGREC_OK;
+}
+
+extern "C" int kgrec_rank_loss_step(const kgrec_tables* tables, int model, const void* pa, const void* pb,
+                                    const void* pc, const void* na, const void* nb, const void* nc, int idx_bytes,
+                                    int64_t n_pos, int32_t n_neg, int64_t batch_pos, int loss_kind,
+                                    float margin_or_target, float grad_loss, const float* gumbel_u, uint64_t seed,
+                                    float* pos_scores, float* neg_scores, float* loss, const kgrec_grads* grads,
+                                    int64_t* slot_user_ids, int64_t* slot_item_ids, int64_t* slot_ent_ids,
+                                    void* workspace, int32_t* status, kgrec_stream_t stream) {
+  return rank_loss_step(tables, model, pa, pb, pc, na, nb, nc, idx_bytes, n_pos, n_neg, batch_pos, loss_kind,
+                        margin_or_target, grad_loss, gumbel_u, seed, pos_scores, neg_scores, loss, grads, slot_user_ids,
+                        slot_item_ids, slot_ent_ids, workspace, status, stream);
+}
+
+extern "C" int kgrec_rank_loss_step_dev(const kgrec_tables* tables, int model, const void* pa, const void* pb,
+                                        const void* pc, const void* na, const void* nb, const void* nc, int idx_bytes,
+                                        int64_t n_pos, int32_t n_neg, int64_t batch_pos, int loss_kind,
+                                        float margin_or_target, float grad_loss, const float* gumbel_u,
+                                        const kgrec_step_state* state, float* pos_scores, float* neg_scores,
+                                        float* loss, const kgrec_grads* grads, int64_t* slot_user_ids,
+                                        int64_t* slot_item_ids, int64_t* slot_ent_ids, void* workspace,
+                                        int32_t* status, kgrec_stream_t stream) {
+  if (!state) { set_error("step state is NULL"); return KGREC_ERR_INVALID; }
+  return rank_loss_step(tables, model, pa, pb, pc, na, nb, nc, idx_bytes, n_pos, n_neg, batch_pos, loss_kind,
+                        margin_or_target, grad_loss, gumbel_u, SeedRef(0, state), pos_scores, neg_scores, loss, grads,
+                        slot_user_ids, slot_item_ids, slot_ent_ids, workspace, status, stream);
 }

@@ -418,12 +418,13 @@ __host__ __device__ inline size_t rec_tables_floats(int P, int d) { return stati
 template <int FAM, int NCH, bool VEC>
 __global__ void __launch_bounds__(kThreads)
 k_score_fwd(const kgrec_tables T, const int ktup, const IdxArgs I, const int64_t n, const float* __restrict__ gumbel_u,
-            const uint64_t seed, float* __restrict__ scores, int32_t* status) {
+            const SeedRef seed_ref, float* __restrict__ scores, int32_t* status) {
   extern __shared__ __align__(16) float smem[];
   const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
   const int64_t first = static_cast<int64_t>(blockIdx.x) * kWarpsPerCta + wid;
   const int64_t step = static_cast<int64_t>(gridDim.x) * kWarpsPerCta;
   if constexpr (FAM == FAM_REC) {
+    const uint64_t seed = seed_ref.get();
     const int stride = (T.dim + 3) & ~3;
     float* sP = smem;
     float* sN = smem + T.n_pref * stride;
@@ -461,7 +462,7 @@ k_score_fwd(const kgrec_tables T, const int ktup, const IdxArgs I, const int64_t
 template <int FAM, int NCH, bool VEC>
 __global__ void __launch_bounds__(kThreads)
 k_rank_loss_fwd(const kgrec_tables T, const int ktup, const IdxArgs I, const LossCfg L,
-                const float* __restrict__ gumbel_u, const uint64_t seed, float* __restrict__ pos_scores,
+                const float* __restrict__ gumbel_u, const SeedRef seed_ref, float* __restrict__ pos_scores,
                 float* __restrict__ neg_scores, float* __restrict__ group_loss, int32_t* status) {
   extern __shared__ __align__(16) float smem[];
   const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
@@ -471,6 +472,7 @@ k_rank_loss_fwd(const kgrec_tables T, const int ktup, const IdxArgs I, const Los
   using R = Row<NCH, VEC>;
   constexpr int NE = NCH * 4;
   if constexpr (FAM == FAM_REC) {
+    const uint64_t seed = seed_ref.get();
     const int stride = (T.dim + 3) & ~3;
     float* sP = smem;
     float* sN = smem + T.n_pref * stride;
@@ -560,7 +562,7 @@ k_rank_loss_fwd(const kgrec_tables T, const int ktup, const IdxArgs I, const Los
 template <int FAM, int NCH, bool VEC, int PR>
 __global__ void __launch_bounds__(kThreads)
 k_score_bwd(const kgrec_tables T, const int ktup, const IdxArgs I, const int64_t n, const LossCfg L,
-            const float* __restrict__ gumbel_u, const uint64_t seed, const BwdArgs B, const kgrec_grads G) {
+            const float* __restrict__ gumbel_u, const SeedRef seed_ref, const BwdArgs B, const kgrec_grads G) {
   extern __shared__ __align__(16) float smem[];
   const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
   const bool fused = B.pos_scores != nullptr;
@@ -568,6 +570,7 @@ k_score_bwd(const kgrec_tables T, const int ktup, const IdxArgs I, const int64_t
   constexpr int NE = NCH * 4;
 
   if constexpr (FAM == FAM_REC) {
+    const uint64_t seed = seed_ref.get();
     const int d = T.dim, P = T.n_pref;
     const int stride = (d + 3) & ~3;
     constexpr int dpad = NCH * 128;
@@ -718,14 +721,14 @@ int set_smem(K kernel, size_t bytes) {
 // return -1 when the shape is outside what it is built for (small n, d > 128, P > 32, unaligned)
 // and the one-warp-per-pair kernels below take the call.
 int rec_tile_score_fwd(const kgrec_tables& T, const Plan& pl, const IdxArgs& I, int64_t n, const float* gumbel_u,
-                       uint64_t seed, float* scores, int32_t* status, cudaStream_t st);
+                       SeedRef seed, float* scores, int32_t* status, cudaStream_t st);
 int rec_tile_rank_loss_fwd(const kgrec_tables& T, const Plan& pl, const IdxArgs& I, const LossCfg& L,
-                           const float* gumbel_u, uint64_t seed, float* pos_scores, float* neg_scores,
+                           const float* gumbel_u, SeedRef seed, float* pos_scores, float* neg_scores,
                            float* group_loss, int32_t* status, cudaStream_t st);
 int rec_tile_score_bwd(const kgrec_tables& T, const Plan& pl, const IdxArgs& I, int64_t n, const LossCfg& L,
-                       const float* gumbel_u, uint64_t seed, const BwdArgs& B, const kgrec_grads& G, cudaStream_t st);
+                       const float* gumbel_u, SeedRef seed, const BwdArgs& B, const kgrec_grads& G, cudaStream_t st);
 int rec_tile_loss_step(const kgrec_tables& T, const Plan& pl, const IdxArgs& I, const LossCfg& L, float grad_loss,
-                       const float* gumbel_u, uint64_t seed, float* pos_scores, float* neg_scores, float* group_loss,
+                       const float* gumbel_u, SeedRef seed, float* pos_scores, float* neg_scores, float* group_loss,
                        const kgrec_grads& G, int64_t* slot_user, int64_t* slot_item, int64_t* slot_ent, int32_t* status,
                        cudaStream_t st);
 int rec_slot_ids(const kgrec_tables& T, const Plan& pl, const IdxArgs& I, int64_t n_pos, int64_t n, int64_t* su, int64_t* si,
@@ -733,7 +736,7 @@ int rec_slot_ids(const kgrec_tables& T, const Plan& pl, const IdxArgs& I, int64_
 
 template <int FAM>
 int launch_score_fwd(const kgrec_tables& T, const Plan& pl, const IdxArgs& I, int64_t n, const float* gumbel_u,
-                     uint64_t seed, float* scores, int32_t* status, cudaStream_t st) {
+                     SeedRef seed, float* scores, int32_t* status, cudaStream_t st) {
   int rc = KGREC_OK;
   if constexpr (FAM == FAM_REC) {
     if ((rc = rec_tile_score_fwd(T, pl, I, n, gumbel_u, seed, scores, status, st)) >= 0) return rc;
@@ -749,7 +752,7 @@ int launch_score_fwd(const kgrec_tables& T, const Plan& pl, const IdxArgs& I, in
 
 template <int FAM>
 int launch_rank_loss_fwd(const kgrec_tables& T, const Plan& pl, const IdxArgs& I, const LossCfg& L,
-                         const float* gumbel_u, uint64_t seed, float* pos_scores, float* neg_scores,
+                         const float* gumbel_u, SeedRef seed, float* pos_scores, float* neg_scores,
                          float* group_loss, int32_t* status, cudaStream_t st) {
   int rc = KGREC_OK;
   if constexpr (FAM == FAM_REC) {
@@ -768,7 +771,7 @@ int launch_rank_loss_fwd(const kgrec_tables& T, const Plan& pl, const IdxArgs& I
 
 template <int FAM>
 int launch_score_bwd(const kgrec_tables& T, const Plan& pl, const IdxArgs& I, int64_t n, const LossCfg& L,
-                     const float* gumbel_u, uint64_t seed, const BwdArgs& B, const kgrec_grads& G, cudaStream_t st) {
+                     const float* gumbel_u, SeedRef seed, const BwdArgs& B, const kgrec_grads& G, cudaStream_t st) {
   int rc = KGREC_OK;
   if constexpr (FAM == FAM_REC) {
     if ((rc = rec_tile_score_bwd(T, pl, I, n, L, gumbel_u, seed, B, G, st)) >= 0) return rc;
@@ -798,10 +801,10 @@ int launch_score_bwd(const kgrec_tables& T, const Plan& pl, const IdxArgs& I, in
 
 #define KGREC_INSTANTIATE_FAMILY(FAMV)                                                                            \
   template int launch_score_fwd<FAMV>(const kgrec_tables&, const Plan&, const IdxArgs&, int64_t, const float*,    \
-                                      uint64_t, float*, int32_t*, cudaStream_t);                                  \
+                                      SeedRef, float*, int32_t*, cudaStream_t);                                  \
   template int launch_rank_loss_fwd<FAMV>(const kgrec_tables&, const Plan&, const IdxArgs&, const LossCfg&,       \
-                                          const float*, uint64_t, float*, float*, float*, int32_t*, cudaStream_t); \
+                                          const float*, SeedRef, float*, float*, float*, int32_t*, cudaStream_t); \
   template int launch_score_bwd<FAMV>(const kgrec_tables&, const Plan&, const IdxArgs&, int64_t, const LossCfg&,  \
-                                      const float*, uint64_t, const BwdArgs&, const kgrec_grads&, cudaStream_t);
+                                      const float*, SeedRef, const BwdArgs&, const kgrec_grads&, cudaStream_t);
 
 }  // namespace kgrec

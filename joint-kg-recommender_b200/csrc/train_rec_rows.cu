@@ -24,7 +24,9 @@ namespace {
 constexpr int kRowThreads = 256;
 
 __global__ void __launch_bounds__(256)
-k_rows_compact(const int32_t* __restrict__ marks, int64_t rows, int32_t epoch, int32_t* __restrict__ list, int32_t* __restrict__ count) {
+k_rows_compact(const int32_t* __restrict__ marks, int64_t rows, int32_t epoch_arg, const kgrec_step_state* state,
+               int32_t* __restrict__ list, int32_t* __restrict__ count) {
+  const int32_t epoch = state ? state->epoch : epoch_arg;
   const int lane = threadIdx.x & 31;
   const int64_t warp = (static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x) >> 5;
   const int64_t n_warps = (static_cast<int64_t>(gridDim.x) * blockDim.x) >> 5;
@@ -486,7 +488,7 @@ struct GumbelPairs {
   float *gx_u, *gx_i, *gz_u, *gz_i, *ck_u, *ck_i;
   float *acc_pref, *acc_pref_norm;
   const float* gram;                 // [3][P][P]
-  const float* gumbel_u; uint64_t seed;
+  const float* gumbel_u; SeedRef seed;
   float *pos_scores, *neg_scores, *group_loss;
   int32_t* status;
   kgrec_tables T; int ktup;
@@ -553,9 +555,10 @@ k_gumbel_pairs(const GumbelPairs A) {
         if (kl) sV[m * P + lane] = gumbel_from_uniform(__ldg(A.gumbel_u + pid * P + lane));
       }
     } else {
+      const uint64_t seed = A.seed.get();
       const int n_vals = (K + 1) * P;
       for (int b = lane; 4 * b < n_vals; b += 32) {
-        const uint4 r = philox4(A.seed, static_cast<uint64_t>(j), static_cast<uint32_t>(b));
+        const uint4 r = philox4(seed, static_cast<uint64_t>(j), static_cast<uint32_t>(b));
         const uint32_t w4[4] = {r.x, r.y, r.z, r.w};
 #pragma unroll
         for (int t = 0; t < 4; ++t)
@@ -762,12 +765,12 @@ extern "C" int64_t kgrec_rec_rows_workspace_floats(int64_t n_user, int64_t n_ite
   return n_user * per + n_item * (per + (ktup ? 2 * static_cast<int64_t>(dim) : 0)) + 3 * static_cast<int64_t>(n_pref) * n_pref + 64;
 }
 
-extern "C" int kgrec_rec_rows_step(const kgrec_tables* tables, int model, const void* pu, const void* pi, const void* ni, int idx_bytes,
-                                   int64_t n_pos, int32_t n_neg, int64_t batch_pos, int loss_kind, float margin_or_target,
-                                   float grad_loss, const int32_t* marks_user, const int32_t* marks_item, int32_t epoch,
-                                   float* workspace, int32_t first_use, const kgrec_grads* acc, float* pos_scores,
-                                   float* neg_scores, float* loss, void* loss_workspace, float* norm_reg_loss,
-                                   const float* gumbel_u, uint64_t seed, int32_t* status, kgrec_stream_t stream) {
+static int rec_rows_step(const kgrec_tables* tables, int model, const void* pu, const void* pi, const void* ni, int idx_bytes,
+                         int64_t n_pos, int32_t n_neg, int64_t batch_pos, int loss_kind, float margin_or_target,
+                         float grad_loss, const int32_t* marks_user, const int32_t* marks_item, int32_t epoch,
+                         const kgrec_step_state* state, float* workspace, int32_t first_use, const kgrec_grads* acc,
+                         float* pos_scores, float* neg_scores, float* loss, void* loss_workspace, float* norm_reg_loss,
+                         const float* gumbel_u, uint64_t seed, int32_t* status, kgrec_stream_t stream) {
   if (!tables || (model != KGREC_TUP && model != KGREC_KTUP)) { set_error("rec_rows_step: TUP / KTUP"); return KGREC_ERR_INVALID; }
   const kgrec_tables& T = *tables;
   const int d = T.dim, P = T.n_pref;
@@ -828,8 +831,8 @@ extern "C" int kgrec_rec_rows_step(const kgrec_tables* tables, int model, const 
     GU.gx = acc->user;
     if (ktup) { GI.ent = T.ent; GI.item2ent = T.item2ent; GI.n_ent = T.n_ent; GI.gx = gxb; GI.acc_table = acc->item; GI.acc_ent = acc->ent; }
     else GI.gx = acc->item;
-    k_rows_compact<<<grid1((nu + 255) / 256), 256, 0, st>>>(marks_user, nu, epoch, gl_u, gcnt);
-    k_rows_compact<<<grid1((nit + 255) / 256), 256, 0, st>>>(marks_item, nit, epoch, gl_i, gcnt + 1);
+    k_rows_compact<<<grid1((nu + 255) / 256), 256, 0, st>>>(marks_user, nu, epoch, state, gl_u, gcnt);
+    k_rows_compact<<<grid1((nit + 255) / 256), 256, 0, st>>>(marks_item, nit, epoch, state, gl_i, gcnt + 1);
     k_gumbel_gram<<<(P * P * 32 + 255) / 256, 256, 0, st>>>(T, ktup ? 1 : 0, gram);
     KGREC_CUDA_OK(cudaGetLastError());
     GumbelPairs A{};
@@ -840,7 +843,7 @@ extern "C" int kgrec_rec_rows_step(const kgrec_tables* tables, int model, const 
     A.a_u = GU.a; A.cn_u = GU.cn; A.a_i = GI.a; A.cn_i = GI.cn;
     A.gx_u = acc->user; A.gx_i = GI.gx; A.gz_u = GU.gz; A.gz_i = GI.gz;
     A.ck_u = GU.ck; A.ck_i = GI.ck;
-    A.acc_pref = acc->pref; A.acc_pref_norm = acc->pref_norm; A.gram = gram; A.gumbel_u = gumbel_u; A.seed = seed;
+    A.acc_pref = acc->pref; A.acc_pref_norm = acc->pref_norm; A.gram = gram; A.gumbel_u = gumbel_u; A.seed = SeedRef(seed, state);
     A.pos_scores = pos_scores; A.neg_scores = neg_scores; A.group_loss = static_cast<float*>(loss_workspace);
     A.status = status; A.T = T; A.ktup = ktup ? 1 : 0;
     A.reg_loss = norm_reg_loss; A.reg_scale = 1.f;
@@ -891,8 +894,8 @@ extern "C" int kgrec_rec_rows_step(const kgrec_tables* tables, int model, const 
   } else {
     I.gx = acc->item;
   }
-  k_rows_compact<<<grid1((nu + 255) / 256), 256, 0, st>>>(marks_user, nu, epoch, list_u, counts);
-  k_rows_compact<<<grid1((nit + 255) / 256), 256, 0, st>>>(marks_item, nit, epoch, list_i, counts + 1);
+  k_rows_compact<<<grid1((nu + 255) / 256), 256, 0, st>>>(marks_user, nu, epoch, state, list_u, counts);
+  k_rows_compact<<<grid1((nit + 255) / 256), 256, 0, st>>>(marks_item, nit, epoch, state, list_i, counts + 1);
   KGREC_CUDA_OK(cudaGetLastError());
 #define ROWS_FWD(PTV)                                                                                                    \
   {                                                                                                                      \
@@ -933,4 +936,28 @@ extern "C" int kgrec_rec_rows_step(const kgrec_tables* tables, int model, const 
   k_batch_loss<<<static_cast<unsigned>(n_batches), 256, 0, st>>>(A.group_loss, A.L, loss);
   KGREC_CUDA_OK(cudaGetLastError());
   return KGREC_OK;
+}
+
+extern "C" int kgrec_rec_rows_step(const kgrec_tables* tables, int model, const void* pu, const void* pi, const void* ni, int idx_bytes,
+                                   int64_t n_pos, int32_t n_neg, int64_t batch_pos, int loss_kind, float margin_or_target,
+                                   float grad_loss, const int32_t* marks_user, const int32_t* marks_item, int32_t epoch,
+                                   float* workspace, int32_t first_use, const kgrec_grads* acc, float* pos_scores,
+                                   float* neg_scores, float* loss, void* loss_workspace, float* norm_reg_loss,
+                                   const float* gumbel_u, uint64_t seed, int32_t* status, kgrec_stream_t stream) {
+  return rec_rows_step(tables, model, pu, pi, ni, idx_bytes, n_pos, n_neg, batch_pos, loss_kind, margin_or_target, grad_loss,
+                       marks_user, marks_item, epoch, nullptr, workspace, first_use, acc, pos_scores, neg_scores, loss,
+                       loss_workspace, norm_reg_loss, gumbel_u, seed, status, stream);
+}
+
+extern "C" int kgrec_rec_rows_step_dev(const kgrec_tables* tables, int model, const void* pu, const void* pi, const void* ni,
+                                       int idx_bytes, int64_t n_pos, int32_t n_neg, int64_t batch_pos, int loss_kind,
+                                       float margin_or_target, float grad_loss, const int32_t* marks_user,
+                                       const int32_t* marks_item, const kgrec_step_state* state, float* workspace,
+                                       int32_t first_use, const kgrec_grads* acc, float* pos_scores, float* neg_scores,
+                                       float* loss, void* loss_workspace, float* norm_reg_loss, const float* gumbel_u,
+                                       int32_t* status, kgrec_stream_t stream) {
+  if (!state) { set_error("rec_rows_step: step state is NULL"); return KGREC_ERR_INVALID; }
+  return rec_rows_step(tables, model, pu, pi, ni, idx_bytes, n_pos, n_neg, batch_pos, loss_kind, margin_or_target, grad_loss,
+                       marks_user, marks_item, 0, state, workspace, first_use, acc, pos_scores, neg_scores, loss,
+                       loss_workspace, norm_reg_loss, gumbel_u, 0, status, stream);
 }

@@ -37,7 +37,7 @@ struct TileArgs {
   int is64;
   int64_t n, n_pos;
   const float* gumbel_u;
-  uint64_t seed;
+  SeedRef seed;
   float *scores_a, *scores_b;    // forward: i < n_pos -> scores_a[i], else scores_b[i - n_pos]
   int32_t* status;
   LossCfg L;                     // backward
@@ -115,6 +115,7 @@ __global__ void __launch_bounds__(kMaxWarps * 32, 1) k_rec_tile(const TileArgs A
   const kgrec_tables& T = A.T;
   const int d = T.dim, P = T.n_pref, NC = d >> 2, lda4 = A.lda >> 2;
   const float hf = A.ktup ? 0.5f : 1.f;
+  const uint64_t seed = GUMBEL ? A.seed.get() : 0;
   const int l1 = T.l1;
 
   float4* sP = reinterpret_cast<float4*>(smem);                       // [NC][PT]   (KTUP: pref + rel)
@@ -280,7 +281,7 @@ __global__ void __launch_bounds__(kMaxWarps * 32, 1) k_rec_tile(const TileArgs A
           nz[j] = 0.f;
           if (k < P && pid >= 0)
             nz[j] = A.gumbel_u ? gumbel_from_uniform(__ldg(A.gumbel_u + pid * P + k))
-                               : gumbel_fast(philox_uniform_bits(A.seed, static_cast<uint64_t>(pid), static_cast<uint32_t>(k)));
+                               : gumbel_fast(philox_uniform_bits(seed, static_cast<uint64_t>(pid), static_cast<uint32_t>(k)));
         }
         float best = -INFINITY;
 #pragma unroll
@@ -654,7 +655,7 @@ int launch_tiles(const TileArgs& A, const TilePlan& tp, cudaStream_t st) {
 
 // ---- entry points used by the FAM_REC launchers (train_dev.cuh); return -1 = not taken ----
 int rec_tile_score_fwd(const kgrec_tables& T, const Plan& pl, const IdxArgs& I, int64_t n, const float* gumbel_u,
-                       uint64_t seed, float* scores, int32_t* status, cudaStream_t st) {
+                       SeedRef seed, float* scores, int32_t* status, cudaStream_t st) {
   TilePlan tp;
   if (!plan_tiles(T, pl, n, kPairsPerWarp, &tp)) return -1;
   TileArgs A{};
@@ -665,7 +666,7 @@ int rec_tile_score_fwd(const kgrec_tables& T, const Plan& pl, const IdxArgs& I, 
 }
 
 int rec_tile_rank_loss_fwd(const kgrec_tables& T, const Plan& pl, const IdxArgs& I, const LossCfg& L,
-                           const float* gumbel_u, uint64_t seed, float* pos_scores, float* neg_scores,
+                           const float* gumbel_u, SeedRef seed, float* pos_scores, float* neg_scores,
                            float* group_loss, int32_t* status, cudaStream_t st) {
   TilePlan tp;
   const int64_t n = L.n_pos * (1 + static_cast<int64_t>(L.n_neg));
@@ -682,7 +683,7 @@ int rec_tile_rank_loss_fwd(const kgrec_tables& T, const Plan& pl, const IdxArgs&
 }
 
 int rec_tile_score_bwd(const kgrec_tables& T, const Plan& pl, const IdxArgs& I, int64_t n, const LossCfg& L,
-                       const float* gumbel_u, uint64_t seed, const BwdArgs& B, const kgrec_grads& G, cudaStream_t st) {
+                       const float* gumbel_u, SeedRef seed, const BwdArgs& B, const kgrec_grads& G, cudaStream_t st) {
   TilePlan tp;
   if (!plan_tiles(T, pl, n, kPairsPerWarp, &tp)) return -1;
   const bool fused = B.pos_scores != nullptr;
@@ -695,7 +696,7 @@ int rec_tile_score_bwd(const kgrec_tables& T, const Plan& pl, const IdxArgs& I, 
 
 // forward + ranking loss + backward in one pass over groups of (positive, its negatives)
 int rec_tile_loss_step(const kgrec_tables& T, const Plan& pl, const IdxArgs& I, const LossCfg& L, float grad_loss,
-                       const float* gumbel_u, uint64_t seed, float* pos_scores, float* neg_scores, float* group_loss,
+                       const float* gumbel_u, SeedRef seed, float* pos_scores, float* neg_scores, float* group_loss,
                        const kgrec_grads& G, int64_t* slot_user, int64_t* slot_item, int64_t* slot_ent, int32_t* status,
                        cudaStream_t st) {
   if (L.n_neg > kPairsPerWarp - 1) return -1;

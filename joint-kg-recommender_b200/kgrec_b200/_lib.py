@@ -52,6 +52,13 @@ class MarkSeg(C.Structure):           # struct kgrec_mark_seg
     ]
 
 
+class StepState(C.Structure):         # struct kgrec_step_state (lives in device memory)
+    _fields_ = [
+        ("step", C.c_int64), ("gumbel_seed", C.c_uint64), ("sample_seed", C.c_uint64), ("epoch", C.c_int32),
+        ("lr", C.c_float),
+    ]
+
+
 _SIGNATURES = {
     "kgrec_abi_version": (C.c_int, []),
     "kgrec_last_error": (C.c_char_p, []),
@@ -101,6 +108,26 @@ _SIGNATURES = {
                                       C.c_int64, C.c_int, C.c_float, C.c_float, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p,
                                       C.c_int32, C.POINTER(Grads), C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                       C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p]),
+    "kgrec_step_advance": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p]),
+    "kgrec_batch_gather": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.c_int,
+                                     C.c_int, C.c_int64, C.c_int64, C.c_void_p, C.c_void_p]),
+    "kgrec_rows_mark_dev": (C.c_int, [C.POINTER(MarkSeg), C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "kgrec_rows_sqnorm_dev": (C.c_int, [C.POINTER(OptTable), C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "kgrec_rows_update_dev": (C.c_int, [C.POINTER(OptTable), C.c_int, C.c_void_p, C.c_int, C.c_float, C.c_float, C.c_float,
+                                        C.c_float, C.c_void_p, C.c_float, C.c_void_p]),
+    "kgrec_sample_corrupt_dev": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int64, C.c_int32, C.c_int64,
+                                           C.c_int64, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "kgrec_sample_neg_items_dev": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int64, C.c_int32, C.c_int64,
+                                             C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "kgrec_rank_loss_step_dev": (C.c_int, [C.POINTER(Tables), C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
+                                           C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int64, C.c_int32,
+                                           C.c_int64, C.c_int, C.c_float, C.c_float, C.c_void_p, C.c_void_p,
+                                           C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(Grads), C.c_void_p, C.c_void_p,
+                                           C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "kgrec_rec_rows_step_dev": (C.c_int, [C.POINTER(Tables), C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int64,
+                                          C.c_int32, C.c_int64, C.c_int, C.c_float, C.c_float, C.c_void_p, C.c_void_p,
+                                          C.c_void_p, C.c_void_p, C.c_int32, C.POINTER(Grads), C.c_void_p, C.c_void_p,
+                                          C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "kgrec_reg_norm_rows": (C.c_int, [C.c_void_p, C.c_int64, C.c_int32, C.c_void_p, C.c_int, C.c_int64, C.c_float,
                                       C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "kgrec_reg_orth_tables": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_int32, C.c_float, C.c_void_p, C.c_void_p,

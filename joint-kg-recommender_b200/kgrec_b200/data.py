@@ -131,6 +131,10 @@ class DeviceTrainIterator:
     def batches_per_epoch(self):
         return max(0, (self.n - self.batch_size)) // self.batch_size + 1
 
+    def batches_left(self):
+        """Batches __next__ yields before it starts a new epoch (host arithmetic only, nothing is read back)."""
+        return max(0, (self.n - self.batch_size - self.start) // self.batch_size)
+
     def __iter__(self):
         return self
 

@@ -63,15 +63,20 @@ class SparseRowOptimizer:
                             n_remap=remap.numel() if remap is not None else 0,
                             marks=m.data_ptr(), rows=m.numel())
 
-    def _mark(self, segs):
-        """Start a step: bump the epoch and mark the rows the step's id arrays name."""
+    def _mark(self, segs, state=None):
+        """Start a step: bump the epoch and mark the rows the step's id arrays name.  state: the epoch is the device
+        step state's (which the caller has advanced for this step); self.t still counts the step."""
         m = self.model
         self.t += 1
         seg_arr = (_lib.MarkSeg * len(segs))(*segs)
-        _lib.check(_lib.load().kgrec_rows_mark(seg_arr, len(segs), self.t, KF._ptr(m._status_buf(m.device)), KF._stream()))
+        status = KF._ptr(m._status_buf(m.device))
+        if state is None:
+            _lib.check(_lib.load().kgrec_rows_mark(seg_arr, len(segs), self.t, status, KF._stream()))
+        else:
+            _lib.check(_lib.load().kgrec_rows_mark_dev(seg_arr, len(segs), state.ptr, status, KF._stream()))
         KF.count_launches(1)
 
-    def _update(self, tables):
+    def _update(self, tables, state=None):
         """Finish a step: total norm (clip) and the optimizer update of the marked rows of `tables`."""
         m = self.model
         lib = _lib.load()
@@ -89,16 +94,23 @@ class SparseRowOptimizer:
         use_clip = self.clip is not None
         if use_clip:
             self.sqnorm.zero_()
-            _lib.check(lib.kgrec_rows_sqnorm(tab_arr, len(entries), self.t, KF._ptr(self.sqnorm), stream))
-        _lib.check(lib.kgrec_rows_update(tab_arr, len(entries), self.t, self.kind, self.lr, self.eps, self.betas[0],
-                                         self.betas[1], self.t, self.wd, KF._ptr(self.sqnorm) if use_clip else None,
-                                         float(self.clip or 0.0), stream))
+            if state is None:
+                _lib.check(lib.kgrec_rows_sqnorm(tab_arr, len(entries), self.t, KF._ptr(self.sqnorm), stream))
+            else:
+                _lib.check(lib.kgrec_rows_sqnorm_dev(tab_arr, len(entries), state.ptr, KF._ptr(self.sqnorm), stream))
+        sq = KF._ptr(self.sqnorm) if use_clip else None
+        if state is None:
+            _lib.check(lib.kgrec_rows_update(tab_arr, len(entries), self.t, self.kind, self.lr, self.eps, self.betas[0],
+                                             self.betas[1], self.t, self.wd, sq, float(self.clip or 0.0), stream))
+        else:      # epoch, lr and Adam's step from the device step state
+            _lib.check(lib.kgrec_rows_update_dev(tab_arr, len(entries), state.ptr, self.kind, self.eps, self.betas[0],
+                                                 self.betas[1], self.wd, sq, float(self.clip or 0.0), stream))
         KF.count_launches(1 + int(use_clip))
 
-    def _apply(self, segs, tables):
+    def _apply(self, segs, tables, state=None):
         """segs: MarkSeg list of this step's id arrays; tables: names of the tables the step's loss reaches."""
-        self._mark(segs)
-        self._update(tables)
+        self._mark(segs, state)
+        self._update(tables, state)
 
     def _grads(self, names):
         g = _lib.Grads()
@@ -108,11 +120,13 @@ class SparseRowOptimizer:
         return g
 
     # -- KG models: TransE / TransH / TransR, and the KG branch of KTUP ---------------------------------
-    def step_corrupt(self, pos, corrupt, margin=1.0, loss="margin", batch_pos=None, reg=False, grad_loss=1.0):
+    def step_corrupt(self, pos, corrupt, margin=1.0, loss="margin", batch_pos=None, reg=False, grad_loss=1.0, state=None):
         """One training step on positives (h, t, r) and group-compact negatives; returns the
         per-batch losses (device tensor; nothing synchronises).  reg=True adds the KG drivers'
         normLoss / orthogonalLoss regularisers inside the same kernel (kgrec_corrupt_loss_step).
-        KTUP: the joint model's KG branch (TransH on ent / rel / norm), grad_loss = kg_lambda."""
+        KTUP: the joint model's KG branch (TransH on ent / rel / norm), grad_loss = kg_lambda.
+        state (kgrec_b200.train.StepState, advanced for this step): the optimizer reads its epoch mark, learning rate
+        and step count on the device (the `_dev` entry points) -- the step a GraphedTrainLoop captures."""
         m = self.model
         if m.MODEL not in (_lib.TRANSE, _lib.TRANSH, _lib.TRANSR, _lib.KTUP):
             raise NotImplementedError("step_corrupt: KG models and the KG branch of KTUP")
@@ -146,17 +160,19 @@ class SparseRowOptimizer:
         KF.count_launches(2)
         segs = [self._seg(pos[0], "ent"), self._seg(pos[1], "ent"), self._seg(corrupt, "ent", compact=True)]
         segs += [self._seg(pos[2], k) for k in ("rel", "norm") if k in names and k in self.marks]   # KTUP: small tables, all rows
-        self._apply(segs, names)
+        self._apply(segs, names, state)
         return out
 
     # -- recommendation models: TUP, and the rec branch of KTUP -----------------------------------------------
-    def step_pairs(self, pos, neg, target=-1.0, loss="bpr", batch_pos=None, gumbel_u=None, reg=False):
+    def step_pairs(self, pos, neg, target=-1.0, loss="bpr", batch_pos=None, gumbel_u=None, reg=False, state=None):
         """One training step on (u, i) positives and (u repeated, ni) negatives: forward + ranking
         loss + backward in the tile kernel (kgrec_rank_loss_step), then clip + update.  reg=True adds
         the driver's regularisers: TUP (item_recommendation.py:177-180) orthogonalLoss(pref, pref_norm) +
         normLoss(user rows) + normLoss(item rows of cat[pos, neg]) + normLoss(pref); KTUP rec branch
         (knowledgable_recommendation.py:343-344) orthogonalLoss(pref, pref_norm).
-        Returns (loss per batch, regulariser value) as device tensors."""
+        Returns (loss per batch, regulariser value) as device tensors.
+        state: as step_corrupt; the Gumbel seed is then state.gumbel_seed + state.step, read on the device, instead of
+        the model's next seed."""
         m = self.model
         if m.MODEL not in (_lib.TUP, _lib.KTUP):
             raise NotImplementedError("step_pairs: TUP / KTUP")
@@ -187,33 +203,40 @@ class SparseRowOptimizer:
         kind = {"margin": _lib.LOSS_MARGIN, "bpr": _lib.LOSS_BPR}[loss]
         if gumbel_u is not None:
             gumbel_u = gumbel_u.to(dev, torch.float32).contiguous()
-        seed = m._next_seed() if (m.use_st_gumbel and gumbel_u is None) else 0
+        seed = m._next_seed() if (m.use_st_gumbel and gumbel_u is None and state is None) else 0
         segs = [self._seg(pu, "user"), self._seg(pi, "item"), self._seg(ni, "item")]
         if ktup:
             segs += [self._seg(pi, "ent", remap=m._item2ent), self._seg(ni, "ent", remap=m._item2ent)]
-        self._mark(segs)
+        self._mark(segs, state)
         rows_path = self._use_rows_path(n_pos, n_neg, nu, pu)
         if rows_path:
             # soft preferences: the [P x d] contractions once per distinct row of the step (csrc/train_rec_rows.cu)
             if self._rows_ws is None:
                 n_fl = lib.kgrec_rec_rows_workspace_floats(w["user"].shape[0], w["item"].shape[0], m.embedding_size,
                                                            w["pref"].shape[0], 1 if ktup else 0)
-                self._rows_ws = torch.empty(int(n_fl), dtype=torch.float32, device=dev)
-                first = 1
+                # device-state steps start from a zeroed workspace instead of first_use: a captured first_use would
+                # clear the accumulators again on every replay
+                self._rows_ws = (torch.empty if state is None else torch.zeros)(int(n_fl), dtype=torch.float32, device=dev)
+                first = int(state is None)
             else:
                 first = 0
-            _lib.check(lib.kgrec_rec_rows_step(
-                C.byref(T), m.MODEL, ptr(pu), ptr(pi), ptr(ni), idx_bytes, n_pos, n_neg, bp, kind, float(target), 1.0,
-                ptr(self.marks["user"]), ptr(self.marks["item"]), self.t, ptr(self._rows_ws), first, C.byref(g),
-                ptr(pos_s), ptr(neg_s), ptr(out), ptr(ws),
-                ptr(self.reg_loss) if (reg and not ktup) else None,
-                ptr(gumbel_u), seed, ptr(m._status_buf(dev)), stream))
+            head = (C.byref(T), m.MODEL, ptr(pu), ptr(pi), ptr(ni), idx_bytes, n_pos, n_neg, bp, kind, float(target), 1.0,
+                    ptr(self.marks["user"]), ptr(self.marks["item"]))
+            tail = (ptr(self._rows_ws), first, C.byref(g), ptr(pos_s), ptr(neg_s), ptr(out), ptr(ws),
+                    ptr(self.reg_loss) if (reg and not ktup) else None, ptr(gumbel_u))
+            if state is None:
+                _lib.check(lib.kgrec_rec_rows_step(*head, self.t, *tail, seed, ptr(m._status_buf(dev)), stream))
+            else:
+                _lib.check(lib.kgrec_rec_rows_step_dev(*head, state.ptr, *tail, ptr(m._status_buf(dev)), stream))
             KF.count_launches(8)
         else:
-            _lib.check(lib.kgrec_rank_loss_step(
-                C.byref(T), m.MODEL, ptr(pu), ptr(pi), None, ptr(nu), ptr(ni), None, idx_bytes, n_pos, n_neg, bp, kind,
-                float(target), 1.0, ptr(gumbel_u), seed, ptr(pos_s), ptr(neg_s), ptr(out), C.byref(g),
-                None, None, None, ptr(ws), ptr(m._status_buf(dev)), stream))
+            head = (C.byref(T), m.MODEL, ptr(pu), ptr(pi), None, ptr(nu), ptr(ni), None, idx_bytes, n_pos, n_neg, bp, kind,
+                    float(target), 1.0, ptr(gumbel_u))
+            tail = (ptr(pos_s), ptr(neg_s), ptr(out), C.byref(g), None, None, None, ptr(ws), ptr(m._status_buf(dev)), stream)
+            if state is None:
+                _lib.check(lib.kgrec_rank_loss_step(*head, seed, *tail))
+            else:
+                _lib.check(lib.kgrec_rank_loss_step_dev(*head, state.ptr, *tail))
             KF.count_launches(2)
         if ktup:      # (pref + rel) and (pref_norm + norm) enter the score as sums (jTransUP.py:253-258): equal gradients
             self.acc["rel"].copy_(self.acc["pref"])
@@ -233,7 +256,7 @@ class SparseRowOptimizer:
                 _lib.check(lib.kgrec_reg_norm_rows(ptr(pw), pw.shape[0], d, None, 8, pw.shape[0], 1.0, ptr(self.reg_loss),
                                                    ptr(self.acc["pref"]), None, stream))
                 KF.count_launches(4)
-        self._update(names)
+        self._update(names, state)
         return out, self.reg_loss
 
     def _use_rows_path(self, n_pos, n_neg, nu, pu):

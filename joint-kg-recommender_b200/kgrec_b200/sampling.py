@@ -49,15 +49,21 @@ class TripleNegativeSampler(_Checked):
             keys = (k[:, 0] * self.n_rel + k[:, 2]) * self.n_ent + k[:, 1]
             self.known = _KnownSet(keys, self.device)
 
-    def sample(self, pos, n_neg, seed):
-        """pos = (h, t, r) device index tensors -> int32 [len(h) * n_neg] corrupt ids."""
+    def sample(self, pos, n_neg, seed=0, state=None):
+        """pos = (h, t, r) device index tensors -> int32 [len(h) * n_neg] corrupt ids.
+        state (kgrec_b200.train.StepState): draw with the running step's seed, state.sample_seed + state.step, read on
+        the device (kgrec_sample_corrupt_dev); `seed` is then not used."""
         h, t, r = (KF.as_index(x, self.device) for x in pos)
         out = torch.empty(h.numel() * n_neg, dtype=torch.int32, device=self.device)
         tab = self.known
-        _lib.check(_lib.load().kgrec_sample_corrupt(
-            KF._ptr(h), KF._ptr(t), KF._ptr(r), KF._idx_bytes(h, t, r), h.numel(), n_neg, self.n_ent, self.n_rel,
-            KF._ptr(tab.table) if tab else None, tab.capacity if tab else 0, int(seed) & 0xFFFFFFFFFFFFFFFF,
-            KF._ptr(out), KF._ptr(self._status()), KF._stream()))
+        lib = _lib.load()
+        args = (KF._ptr(h), KF._ptr(t), KF._ptr(r), KF._idx_bytes(h, t, r), h.numel(), n_neg, self.n_ent, self.n_rel,
+                KF._ptr(tab.table) if tab else None, tab.capacity if tab else 0)
+        tail = (KF._ptr(out), KF._ptr(self._status()), KF._stream())
+        if state is None:
+            _lib.check(lib.kgrec_sample_corrupt(*args, int(seed) & 0xFFFFFFFFFFFFFFFF, *tail))
+        else:
+            _lib.check(lib.kgrec_sample_corrupt_dev(*args, state.ptr, *tail))
         KF.count_launches(1)
         return out
 
@@ -77,13 +83,18 @@ class RatingNegativeSampler(_Checked):
             k = torch.as_tensor(known_ratings, dtype=torch.int64)
             self.known = _KnownSet(k[:, 0] * self.n_item + k[:, 1], self.device)
 
-    def sample(self, u, pi, n_neg, seed):
+    def sample(self, u, pi, n_neg, seed=0, state=None):
+        """state: as TripleNegativeSampler.sample (kgrec_sample_neg_items_dev)."""
         u, pi = KF.as_index(u, self.device), KF.as_index(pi, self.device)
         out = torch.empty(u.numel() * n_neg, dtype=torch.int32, device=self.device)
         tab = self.known
-        _lib.check(_lib.load().kgrec_sample_neg_items(
-            KF._ptr(u), KF._ptr(pi), KF._idx_bytes(u, pi), u.numel(), n_neg, self.n_item,
-            KF._ptr(tab.table) if tab else None, tab.capacity if tab else 0, int(seed) & 0xFFFFFFFFFFFFFFFF,
-            KF._ptr(out), KF._ptr(self._status()), KF._stream()))
+        lib = _lib.load()
+        args = (KF._ptr(u), KF._ptr(pi), KF._idx_bytes(u, pi), u.numel(), n_neg, self.n_item,
+                KF._ptr(tab.table) if tab else None, tab.capacity if tab else 0)
+        tail = (KF._ptr(out), KF._ptr(self._status()), KF._stream())
+        if state is None:
+            _lib.check(lib.kgrec_sample_neg_items(*args, int(seed) & 0xFFFFFFFFFFFFFFFF, *tail))
+        else:
+            _lib.check(lib.kgrec_sample_neg_items_dev(*args, state.ptr, *tail))
         KF.count_launches(1)
         return out
