@@ -370,6 +370,40 @@ int kgrec_rows_sqnorm_dev(const kgrec_opt_table* tabs_host, int n_tabs, const kg
 int kgrec_rows_update_dev(const kgrec_opt_table* tabs_host, int n_tabs, const kgrec_step_state* state, int kind,
                           float eps, float beta1, float beta2, float weight_decay, const float* sqnorm,
                           float max_norm, kgrec_stream_t stream);
+
+/* ---- exact torch.optim trajectories (utils/trainer.py:63-102) ------------------------------------
+ * kgrec_rows_update with every rule of the reference's trainer and its dense row semantics.  Rules are
+ * torch.optim's formulas; weight decay is added to the clipped gradient:
+ *   kind 0 SGD      state1 = momentum buffer (momentum != 0):  buf = mu buf + g ; p -= lr buf
+ *   kind 1 Adagrad  state1 = sum
+ *   kind 2 Adam     state1 = m, state2 = v; the bias terms use step_counts[t], the step count of table t
+ *                   of the call, which the call advances by one (in the stream, before the sweep) -- as
+ *                   torch advances a parameter's step only when the parameter has a gradient
+ *   kind 3 RMSprop  (centered = False) state1 = square_avg, state2 = momentum buffer (momentum != 0):
+ *                   sq = alpha sq + (1 - alpha) g^2 ; p -= lr g / (sqrt(sq) + eps)  (or via the buffer)
+ * rows: KGREC_ROWS_TOUCHED updates the marked rows (as kgrec_rows_update); KGREC_ROWS_ALL updates every
+ * row of every table of the call, as torch.optim's dense step does: a marked row with its clipped
+ * accumulator (then cleared), an unmarked row with gradient 0 (its accumulator is not read).  It costs
+ * O(table) per call.  Plain SGD and Adagrad without weight decay leave a zero-gradient row bit-unchanged,
+ * so for them ALL visits the marked rows only. */
+enum { KGREC_ROWS_TOUCHED = 0, KGREC_ROWS_ALL = 1 };
+typedef struct kgrec_opt_params {
+  int32_t kind;          /* 0 SGD, 1 Adagrad, 2 Adam, 3 RMSprop                                    */
+  int32_t rows;          /* KGREC_ROWS_TOUCHED | KGREC_ROWS_ALL                                    */
+  float lr;              /* kgrec_rows_update_ex only (_ex_dev reads state->lr)                    */
+  float eps;
+  float beta1, beta2;    /* Adam                                                                   */
+  float alpha;           /* RMSprop                                                                */
+  float momentum;        /* SGD, RMSprop (0: no buffer)                                            */
+  float weight_decay;
+  float max_norm;        /* clip, when sqnorm is given                                             */
+  int64_t* step_counts;  /* [n_tabs] int64 device counters, one per table of the call (Adam)       */
+} kgrec_opt_params;
+int kgrec_rows_update_ex(const kgrec_opt_table* tabs_host, int n_tabs, int32_t epoch, const kgrec_opt_params* params_host,
+                         const float* sqnorm, kgrec_stream_t stream);
+/* the same with the epoch and the learning rate read from *state (a CUDA-graph-capturable step) */
+int kgrec_rows_update_ex_dev(const kgrec_opt_table* tabs_host, int n_tabs, const kgrec_step_state* state,
+                             const kgrec_opt_params* params_host, const float* sqnorm, kgrec_stream_t stream);
 /* the samplers with seed = state->sample_seed + state->step */
 int kgrec_sample_corrupt_dev(const void* ph, const void* pt, const void* pr, int idx_bytes, int64_t n_pos,
                              int32_t n_neg, int64_t n_ent, int64_t n_rel, const uint64_t* table, int64_t capacity,

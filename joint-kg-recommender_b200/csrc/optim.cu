@@ -14,11 +14,17 @@
 // processed with 128-bit loads / stores (lane = 16-byte chunk).  Per step the cost is
 // rows * 4 B of marks + touched rows * (2..4 reads + 2..4 writes) of d floats -- at configs[1]
 // (100k entities, every row touched) ~0.25 GB, against ~1.3 GB for the id-list + CAS version it replaces.
+//
+// Exact (torch.optim) trajectories: kgrec_rows_update_ex / _ex_dev add SGD with momentum and RMSprop, per-table Adam
+// step counts, and row mode ALL -- every row of every table of the call is updated, as the reference's dense optimizer
+// does (utils/trainer.py:63-81): a marked row with its clipped accumulator, an unmarked row with gradient 0 (its
+// accumulator is zero and is not read).  ALL is a flat streaming sweep (k_rows_update_all): 128-bit units, several
+// units per thread in flight, one launch for every table.  Its cost is O(table) per step, the reference's own.
 #include "common.cuh"
 
 namespace kgrec {
 
-enum { OPT_SGD = 0, OPT_ADAGRAD = 1, OPT_ADAM = 2 };
+enum { OPT_SGD = 0, OPT_ADAGRAD = 1, OPT_ADAM = 2, OPT_RMSPROP = 3 };
 constexpr int kMaxOptTables = 8;
 constexpr int kMaxMarkSegs = 8;
 
@@ -57,14 +63,18 @@ __global__ void __launch_bounds__(256) k_rows_mark(const MarkArgs A, int32_t* st
 struct SweepArgs {
   kgrec_opt_table tab[kMaxOptTables];
   int64_t chunk_begin[kMaxOptTables + 1];    // prefix sums of ceil(rows / 32)
+  int64_t unit_begin[kMaxOptTables + 1];     // prefix sums of rows * dim / (vec ? 4 : 1): the units of the ALL sweep
   int32_t div[kMaxOptTables];                // sweep rows per table row (wide rows are swept in segments)
   int n_tabs;
   int32_t epoch;
   int kind;
   float lr, eps, beta1, beta2, wd, bias1, bias2_sqrt;
+  float alpha, momentum;                     // RMSprop's smoothing constant; SGD / RMSprop momentum (0: none)
+  int use_s1, use_s2;                        // the rule keeps state1 / state2
   const float* sqnorm;
   float max_norm;
   const kgrec_step_state* state;             // _dev entry points: epoch, lr and Adam's step are read here
+  const int64_t* steps;                      // _ex: Adam's step count per table of the call (NULL: the global step)
 };
 
 // The scalars of one step: the by-value arguments, or the device step state's
@@ -99,14 +109,14 @@ __device__ __forceinline__ void sweep_rows(const SweepArgs& A, int32_t epoch, F&
         rows[i] = row0;
         if (m) { rows[i] = row0 + (__ffs(m) - 1); m &= m - 1; n = i + 1; }
       }
-      f(T, rows, n, lane);
+      f(T, t, rows, n, lane);
     }
   }
 }
 
 __global__ void __launch_bounds__(256) k_rows_sqnorm(const SweepArgs A, float* out) {
   float local = 0.f;
-  sweep_rows(A, sweep_epoch(A), [&](const kgrec_opt_table& T, const int64_t (&rows)[kRowsInFlight], int n, int lane) {
+  sweep_rows(A, sweep_epoch(A), [&](const kgrec_opt_table& T, int, const int64_t (&rows)[kRowsInFlight], int n, int lane) {
     const int nch = (T.dim + 3) >> 2;
     for (int ch = lane; ch < nch; ch += 32) {
       if (T.vec) {
@@ -138,12 +148,26 @@ __global__ void __launch_bounds__(256) k_rows_sqnorm(const SweepArgs A, float* o
 struct StepScalars { float lr, bias1, bias2_sqrt; };
 
 __device__ __forceinline__ float opt_elem(const SweepArgs& A, const StepScalars& S, float pv, float gv, float* s1, float* s2) {
-  if (A.wd != 0.f) gv = fmaf(A.wd, pv, gv);          // weight_decay = l2_lambda, on touched rows only
-  if (A.kind == OPT_SGD) return pv - S.lr * gv;
+  if (A.wd != 0.f) gv = fmaf(A.wd, pv, gv);          // weight_decay = l2_lambda, on the rows the call updates
+  if (A.kind == OPT_SGD) {
+    if (A.momentum == 0.f) return pv - S.lr * gv;
+    const float b = __fmul_rn(A.momentum, *s1) + gv;  // torch.optim.SGD: buf = mu buf + g (a zero buf: g) ; p -= lr buf
+    *s1 = b;
+    return pv - S.lr * b;
+  }
   if (A.kind == OPT_ADAGRAD) {                        // torch.optim.Adagrad: sum += g^2 ; p -= lr g / (sqrt(sum) + eps)
     const float s = fmaf(gv, gv, *s1);
     *s1 = s;
     return pv - S.lr * gv / (sqrtf(s) + A.eps);
+  }
+  if (A.kind == OPT_RMSPROP) {                        // torch.optim.RMSprop, centered=False: sq = a sq + (1 - a) g^2
+    const float sq = fmaf((1.f - A.alpha) * gv, gv, __fmul_rn(A.alpha, *s1));
+    *s1 = sq;
+    const float q = gv / (sqrtf(sq) + A.eps);
+    if (A.momentum == 0.f) return pv - S.lr * q;      // p -= lr g / (sqrt(sq) + eps)
+    const float b = __fmul_rn(A.momentum, *s2) + q;   // buf = mu buf + g / (sqrt(sq) + eps) ; p -= lr buf
+    *s2 = b;
+    return pv - S.lr * b;
   }
   const float m = A.beta1 * *s1 + (1.f - A.beta1) * gv;          // torch.optim.Adam on the touched rows ("lazy")
   const float v = A.beta2 * *s2 + (1.f - A.beta2) * gv * gv;
@@ -152,17 +176,38 @@ __device__ __forceinline__ float opt_elem(const SweepArgs& A, const StepScalars&
   return pv - (S.lr / S.bias1) * m / (sqrtf(v) / S.bias2_sqrt + A.eps);
 }
 
+// Adam's bias terms of every table of the call from its own step count (the _ex entry points), in shared memory
+struct TableBias { float bias1[kMaxOptTables], bias2_sqrt[kMaxOptTables]; };
+
+__device__ __forceinline__ void table_bias(const SweepArgs& A, TableBias& B) {
+  if (threadIdx.x < A.n_tabs) {
+    const float t = static_cast<float>(A.steps[threadIdx.x]);
+    B.bias1[threadIdx.x] = 1.f - powf(A.beta1, t);
+    B.bias2_sqrt[threadIdx.x] = sqrtf(1.f - powf(A.beta2, t));
+  }
+  __syncthreads();
+}
+
+__device__ __forceinline__ StepScalars table_scalars(const SweepArgs& A, const StepScalars& S, const TableBias& B, int t) {
+  float b1 = S.bias1, b2 = S.bias2_sqrt;
+  if (A.steps) { b1 = B.bias1[t]; b2 = B.bias2_sqrt[t]; }
+  return StepScalars{S.lr, b1, b2};
+}
+
 __global__ void __launch_bounds__(256) k_rows_update(const SweepArgs A) {
   float scale = 1.f;
   if (A.sqnorm) scale = fminf(1.f, A.max_norm / (sqrtf(__ldg(A.sqnorm)) + 1e-6f));   // clip_grad_norm's coefficient
-  StepScalars S{A.lr, A.bias1, A.bias2_sqrt};
+  StepScalars S0{A.lr, A.bias1, A.bias2_sqrt};
   if (A.state) {          // the host formulas of kgrec_rows_update, on the device
     const float t = static_cast<float>(A.state->step);
-    S.lr = A.state->lr;
-    S.bias1 = 1.f - powf(A.beta1, t);
-    S.bias2_sqrt = sqrtf(1.f - powf(A.beta2, t));
+    S0.lr = A.state->lr;
+    S0.bias1 = 1.f - powf(A.beta1, t);
+    S0.bias2_sqrt = sqrtf(1.f - powf(A.beta2, t));
   }
-  sweep_rows(A, sweep_epoch(A), [&](const kgrec_opt_table& T, const int64_t (&rows)[kRowsInFlight], int n, int lane) {
+  __shared__ TableBias B;
+  if (A.steps) table_bias(A, B);
+  sweep_rows(A, sweep_epoch(A), [&](const kgrec_opt_table& T, int t, const int64_t (&rows)[kRowsInFlight], int n, int lane) {
+    const StepScalars S = table_scalars(A, S0, B, t);
     const int nch = (T.dim + 3) >> 2;
     const float4 z4 = make_float4(0.f, 0.f, 0.f, 0.f);
     for (int ch = lane; ch < nch; ch += 32) {
@@ -175,8 +220,8 @@ __global__ void __launch_bounds__(256) k_rows_update(const SweepArgs A) {
           if (i < n) {
             g[i] = *reinterpret_cast<const float4*>(T.acc + o);
             p[i] = *reinterpret_cast<const float4*>(T.table + o);
-            if (A.kind != OPT_SGD) a[i] = *reinterpret_cast<const float4*>(T.state1 + o);
-            if (A.kind == OPT_ADAM) b[i] = *reinterpret_cast<const float4*>(T.state2 + o);
+            if (A.use_s1) a[i] = *reinterpret_cast<const float4*>(T.state1 + o);
+            if (A.use_s2) b[i] = *reinterpret_cast<const float4*>(T.state2 + o);
           }
         }
 #pragma unroll
@@ -189,23 +234,105 @@ __global__ void __launch_bounds__(256) k_rows_update(const SweepArgs A) {
           p[i].w = opt_elem(A, S, p[i].w, g[i].w * scale, &a[i].w, &b[i].w);
           if (!T.keep_acc) *reinterpret_cast<float4*>(T.acc + o) = z4;                   // zero again after the step
           *reinterpret_cast<float4*>(T.table + o) = p[i];
-          if (A.kind != OPT_SGD) *reinterpret_cast<float4*>(T.state1 + o) = a[i];
-          if (A.kind == OPT_ADAM) *reinterpret_cast<float4*>(T.state2 + o) = b[i];
+          if (A.use_s1) *reinterpret_cast<float4*>(T.state1 + o) = a[i];
+          if (A.use_s2) *reinterpret_cast<float4*>(T.state2 + o) = b[i];
         }
       } else {
-        for (int i = 0; i < n; ++i)
-          for (int e = 0; e < 4 && ch * 4 + e < T.dim; ++e) {
+#pragma unroll
+        for (int i = 0; i < kRowsInFlight; ++i)
+          for (int e = 0; i < n && e < 4 && ch * 4 + e < T.dim; ++e) {
             const int64_t o = rows[i] * T.dim + ch * 4 + e;
             const float g = T.acc[o];
             if (!T.keep_acc) T.acc[o] = 0.f;
-            float a = A.kind != OPT_SGD ? T.state1[o] : 0.f, b = A.kind == OPT_ADAM ? T.state2[o] : 0.f;
+            float a = A.use_s1 ? T.state1[o] : 0.f, b = A.use_s2 ? T.state2[o] : 0.f;
             T.table[o] = opt_elem(A, S, T.table[o], g * scale, &a, &b);
-            if (A.kind != OPT_SGD) T.state1[o] = a;
-            if (A.kind == OPT_ADAM) T.state2[o] = b;
+            if (A.use_s1) T.state1[o] = a;
+            if (A.use_s2) T.state2[o] = b;
           }
       }
     }
   });
+}
+
+// Row mode ALL: every row of every table.  The tables are one flat array of units -- a float4 (vec tables) or a float
+// (the scalar path) -- walked grid-stride, kAllUnroll units a thread in flight: marks, parameters and state are loaded
+// for all of them, then the accumulators of the marked ones, then the rule runs and everything is stored.  An unmarked
+// row's gradient is 0: its accumulator is neither read nor written.
+constexpr int kAllUnroll = 4;
+
+__device__ __forceinline__ float4 ld_unit(const float* base, int64_t o, bool vec) {
+  return vec ? *reinterpret_cast<const float4*>(base + o) : make_float4(base[o], 0.f, 0.f, 0.f);
+}
+
+__device__ __forceinline__ void st_unit(float* base, int64_t o, bool vec, const float4& v) {
+  if (vec) *reinterpret_cast<float4*>(base + o) = v;
+  else base[o] = v.x;
+}
+
+__global__ void __launch_bounds__(256) k_rows_update_all(const SweepArgs A) {
+  float scale = 1.f;
+  if (A.sqnorm) scale = fminf(1.f, A.max_norm / (sqrtf(__ldg(A.sqnorm)) + 1e-6f));   // clip_grad_norm's coefficient
+  StepScalars S0{A.lr, A.bias1, A.bias2_sqrt};
+  if (A.state) S0.lr = A.state->lr;
+  __shared__ TableBias B;
+  if (A.steps) table_bias(A, B);
+  const int32_t epoch = sweep_epoch(A);
+  const int64_t total = A.unit_begin[A.n_tabs];
+  const int64_t stride = static_cast<int64_t>(gridDim.x) * blockDim.x;
+  const float4 z4 = make_float4(0.f, 0.f, 0.f, 0.f);
+  for (int64_t base = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x; base < total; base += kAllUnroll * stride) {
+    int tab[kAllUnroll];
+    int64_t off[kAllUnroll];
+    bool on[kAllUnroll], marked[kAllUnroll];
+    float4 p[kAllUnroll], a[kAllUnroll], b[kAllUnroll], g[kAllUnroll];
+#pragma unroll
+    for (int i = 0; i < kAllUnroll; ++i) {           // marks, parameters and state of every unit first
+      const int64_t u = base + i * stride;
+      on[i] = u < total;
+      int t = 0;
+#pragma unroll
+      for (int k = 1; k < kMaxOptTables; ++k) t += (k < A.n_tabs && u >= A.unit_begin[k]) ? 1 : 0;
+      tab[i] = t;
+      const kgrec_opt_table& T = A.tab[t];
+      const int64_t local = u - A.unit_begin[t];
+      const int64_t per_row = T.vec ? (T.dim >> 2) : T.dim;
+      const int64_t row = local < 0xFFFFFFFFll ? static_cast<int64_t>(static_cast<uint32_t>(local) / static_cast<uint32_t>(per_row))
+                                               : local / per_row;
+      off[i] = T.vec ? local * 4 : local;
+      marked[i] = false;
+      p[i] = a[i] = b[i] = g[i] = z4;
+      if (on[i]) {
+        marked[i] = !T.marks || __ldg(T.marks + (A.div[t] == 1 ? row : row / A.div[t])) == epoch;
+        p[i] = ld_unit(T.table, off[i], T.vec);
+        if (A.use_s1) a[i] = ld_unit(T.state1, off[i], T.vec);
+        if (A.use_s2) b[i] = ld_unit(T.state2, off[i], T.vec);
+      }
+    }
+#pragma unroll
+    for (int i = 0; i < kAllUnroll; ++i)              // then the gradients of the marked units
+      if (marked[i]) g[i] = ld_unit(A.tab[tab[i]].acc, off[i], A.tab[tab[i]].vec);
+#pragma unroll
+    for (int i = 0; i < kAllUnroll; ++i) {
+      if (!on[i]) continue;
+      const kgrec_opt_table& T = A.tab[tab[i]];
+      const StepScalars S = table_scalars(A, S0, B, tab[i]);
+      p[i].x = opt_elem(A, S, p[i].x, g[i].x * scale, &a[i].x, &b[i].x);
+      if (T.vec) {
+        p[i].y = opt_elem(A, S, p[i].y, g[i].y * scale, &a[i].y, &b[i].y);
+        p[i].z = opt_elem(A, S, p[i].z, g[i].z * scale, &a[i].z, &b[i].z);
+        p[i].w = opt_elem(A, S, p[i].w, g[i].w * scale, &a[i].w, &b[i].w);
+      }
+      if (marked[i] && !T.keep_acc) st_unit(T.acc, off[i], T.vec, z4);
+      st_unit(T.table, off[i], T.vec, p[i]);
+      if (A.use_s1) st_unit(T.state1, off[i], T.vec, a[i]);
+      if (A.use_s2) st_unit(T.state2, off[i], T.vec, b[i]);
+    }
+  }
+}
+
+// Adam's per-table step counts: +1 for every table of the call, ordered in the stream ahead of the sweep that reads them
+__global__ void k_step_counts(int64_t* steps, int n_tabs) {
+  if (threadIdx.x < n_tabs) steps[threadIdx.x] += 1;
 }
 
 }  // namespace kgrec
@@ -238,8 +365,12 @@ static int sweep_args(const kgrec_opt_table* tabs, int n_tabs, int32_t epoch, in
         if (T.dim % seg == 0) { A.div[t] = T.dim / seg; T.rows *= A.div[t]; T.dim = seg; break; }
     A.tab[t] = T;
     A.chunk_begin[t + 1] = A.chunk_begin[t] + (T.rows + 31) / 32;
+    A.unit_begin[t + 1] = A.unit_begin[t] + T.rows * T.dim / (T.vec ? 4 : 1);
   }
-  for (int t = n_tabs; t < kMaxOptTables; ++t) A.chunk_begin[t + 1] = A.chunk_begin[n_tabs];
+  for (int t = n_tabs; t < kMaxOptTables; ++t) {
+    A.chunk_begin[t + 1] = A.chunk_begin[n_tabs];
+    A.unit_begin[t + 1] = A.unit_begin[n_tabs];
+  }
   return KGREC_OK;
 }
 
@@ -301,10 +432,60 @@ static int rows_update(const kgrec_opt_table* tabs, int n_tabs, int32_t epoch, c
       return KGREC_ERR_INVALID;
     }
   A.kind = kind; A.lr = lr; A.eps = eps; A.beta1 = beta1; A.beta2 = beta2; A.wd = weight_decay;
+  A.use_s1 = kind != OPT_SGD;
+  A.use_s2 = kind == OPT_ADAM;
   A.bias1 = 1.f - powf(beta1, static_cast<float>(step));
   A.bias2_sqrt = sqrtf(1.f - powf(beta2, static_cast<float>(step)));
   A.sqnorm = sqnorm; A.max_norm = max_norm; A.state = state;
   k_rows_update<<<sweep_grid(A), 256, 0, static_cast<cudaStream_t>(stream)>>>(A);
+  KGREC_CUDA_OK(cudaGetLastError());
+  return KGREC_OK;
+}
+
+// kgrec_rows_update_ex / _ex_dev: every rule, either row mode, Adam's step count per table
+static int rows_update_ex(const kgrec_opt_table* tabs, int n_tabs, int32_t epoch, const kgrec_step_state* state,
+                          const kgrec_opt_params* P, const float* sqnorm, kgrec_stream_t stream) {
+  if (!P) { set_error("sparse row optimizer: params is NULL"); return KGREC_ERR_INVALID; }
+  SweepArgs A;
+  int rc = sweep_args(tabs, n_tabs, epoch, 1, A);
+  if (rc) return rc;
+  const int kind = P->kind;
+  if (kind < OPT_SGD || kind > OPT_RMSPROP) { set_error("sparse row optimizer: unknown kind %d", kind); return KGREC_ERR_INVALID; }
+  if (P->rows != KGREC_ROWS_TOUCHED && P->rows != KGREC_ROWS_ALL) {
+    set_error("sparse row optimizer: unknown row mode %d", P->rows);
+    return KGREC_ERR_INVALID;
+  }
+  A.use_s1 = kind != OPT_SGD || P->momentum != 0.f;
+  A.use_s2 = kind == OPT_ADAM || (kind == OPT_RMSPROP && P->momentum != 0.f);
+  for (int t = 0; t < n_tabs; ++t)
+    if ((A.use_s1 && !tabs[t].state1) || (A.use_s2 && !tabs[t].state2)) {
+      set_error("sparse row optimizer: state missing for optimizer kind %d, momentum %g (table %d)", kind,
+                static_cast<double>(P->momentum), t);
+      return KGREC_ERR_INVALID;
+    }
+  if (kind == OPT_ADAM && !P->step_counts) {
+    set_error("sparse row optimizer: Adam needs its per-table step counts (step_counts is NULL)");
+    return KGREC_ERR_INVALID;
+  }
+  A.kind = kind; A.lr = P->lr; A.eps = P->eps; A.beta1 = P->beta1; A.beta2 = P->beta2; A.wd = P->weight_decay;
+  A.alpha = P->alpha; A.momentum = P->momentum;
+  A.sqnorm = sqnorm; A.max_norm = P->max_norm; A.state = state; A.steps = P->step_counts;
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
+  if (P->step_counts) {
+    k_step_counts<<<1, 32, 0, s>>>(P->step_counts, n_tabs);
+    KGREC_CUDA_OK(cudaGetLastError());
+  }
+  // a zero gradient leaves a row bit-unchanged under plain SGD and Adagrad without weight decay: ALL then only costs
+  // more, and the marked rows are enough
+  const bool all = P->rows == KGREC_ROWS_ALL &&
+                   !(((kind == OPT_SGD && P->momentum == 0.f) || kind == OPT_ADAGRAD) && P->weight_decay == 0.f);
+  if (all) {
+    const int64_t units = A.unit_begin[n_tabs];
+    const int64_t blocks = (units + 256 * kAllUnroll - 1) / (256 * kAllUnroll), cap = static_cast<int64_t>(sm_count()) * 8;
+    k_rows_update_all<<<static_cast<int>(blocks < 1 ? 1 : (blocks < cap ? blocks : cap)), 256, 0, s>>>(A);
+  } else {
+    k_rows_update<<<sweep_grid(A), 256, 0, s>>>(A);
+  }
   KGREC_CUDA_OK(cudaGetLastError());
   return KGREC_OK;
 }
@@ -342,4 +523,15 @@ extern "C" int kgrec_rows_update_dev(const kgrec_opt_table* tabs, int n_tabs, co
                                      float max_norm, kgrec_stream_t stream) {
   if (!state) { set_error("sparse row optimizer: step state is NULL"); return KGREC_ERR_INVALID; }
   return rows_update(tabs, n_tabs, 0, state, kind, 0.f, eps, beta1, beta2, 1, weight_decay, sqnorm, max_norm, stream);
+}
+
+extern "C" int kgrec_rows_update_ex(const kgrec_opt_table* tabs, int n_tabs, int32_t epoch, const kgrec_opt_params* params,
+                                    const float* sqnorm, kgrec_stream_t stream) {
+  return rows_update_ex(tabs, n_tabs, epoch, nullptr, params, sqnorm, stream);
+}
+
+extern "C" int kgrec_rows_update_ex_dev(const kgrec_opt_table* tabs, int n_tabs, const kgrec_step_state* state,
+                                        const kgrec_opt_params* params, const float* sqnorm, kgrec_stream_t stream) {
+  if (!state) { set_error("sparse row optimizer: step state is NULL"); return KGREC_ERR_INVALID; }
+  return rows_update_ex(tabs, n_tabs, 0, state, params, sqnorm, stream);
 }

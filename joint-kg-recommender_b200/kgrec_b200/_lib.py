@@ -52,6 +52,17 @@ class MarkSeg(C.Structure):           # struct kgrec_mark_seg
     ]
 
 
+class OptParams(C.Structure):         # struct kgrec_opt_params
+    _fields_ = [
+        ("kind", C.c_int32), ("rows", C.c_int32), ("lr", C.c_float), ("eps", C.c_float), ("beta1", C.c_float),
+        ("beta2", C.c_float), ("alpha", C.c_float), ("momentum", C.c_float), ("weight_decay", C.c_float),
+        ("max_norm", C.c_float), ("step_counts", C.c_void_p),
+    ]
+
+
+ROWS_TOUCHED, ROWS_ALL = 0, 1
+
+
 class StepState(C.Structure):         # struct kgrec_step_state (lives in device memory)
     _fields_ = [
         ("step", C.c_int64), ("gumbel_seed", C.c_uint64), ("sample_seed", C.c_uint64), ("epoch", C.c_int32),
@@ -115,6 +126,10 @@ _SIGNATURES = {
     "kgrec_rows_sqnorm_dev": (C.c_int, [C.POINTER(OptTable), C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
     "kgrec_rows_update_dev": (C.c_int, [C.POINTER(OptTable), C.c_int, C.c_void_p, C.c_int, C.c_float, C.c_float, C.c_float,
                                         C.c_float, C.c_void_p, C.c_float, C.c_void_p]),
+    "kgrec_rows_update_ex": (C.c_int, [C.POINTER(OptTable), C.c_int, C.c_int32, C.POINTER(OptParams), C.c_void_p,
+                                       C.c_void_p]),
+    "kgrec_rows_update_ex_dev": (C.c_int, [C.POINTER(OptTable), C.c_int, C.c_void_p, C.POINTER(OptParams), C.c_void_p,
+                                           C.c_void_p]),
     "kgrec_sample_corrupt_dev": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int64, C.c_int32, C.c_int64,
                                            C.c_int64, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "kgrec_sample_neg_items_dev": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int64, C.c_int32, C.c_int64,

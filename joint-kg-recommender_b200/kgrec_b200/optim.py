@@ -17,6 +17,16 @@ only ("lazy"), which differs from dense Adam on untouched rows (SURVEY 7.3-3).  
 part in a step when the step's loss reaches it -- as in the reference, where parameters whose
 ``.grad`` is None are skipped (KTUP: the rec branch moves user / item / aligned entities / pref /
 pref_norm / rel / norm, the KG branch ent / rel / norm).
+
+Exact trajectories (rows="all", kgrec_rows_update_ex): the reference's trainer steps a dense torch.optim optimizer over
+nn.Embedding tables with dense gradients, so every row of every table the loss reaches moves on every step -- Adam
+through m / v, SGD / RMSprop through their momentum buffers, any rule through weight decay -- including rows the batch
+did not touch.  rows="all" does the same, at O(table) per step as the reference does; rows="touched" (the default)
+stays the fast O(batch) mode that is not the reference's trajectory.  Also there: SGD with momentum, RMSprop (the
+reference's "Rmsprop"), Adam's step count per table (torch keeps one per parameter), and reset(), the trainer's
+optimizer_reset.  "A table takes part" is torch >= 2's zero_grad(set_to_none=True) rule above.  The reference was written
+for torch 0.3, whose zero_grad zeroed gradients in place: there KTUP's rec tables, once they have a gradient, also take
+part in KG steps (weight decay and Adam's m / v keep moving them).  That variant is not built.
 """
 import ctypes as C
 
@@ -25,7 +35,10 @@ import torch
 from . import _lib
 from . import functional as KF
 
-_KINDS = {"SGD": 0, "Adagrad": 1, "Adam": 2}
+_KINDS = {"SGD": 0, "Adagrad": 1, "Adam": 2, "Rmsprop": 3, "RMSprop": 3}
+_ROWS = {"touched": _lib.ROWS_TOUCHED, "all": _lib.ROWS_ALL}
+# utils/trainer.py:63-78: the reference's -optimizer_type values; momentum = FLAGS.momentum for SGD and Rmsprop only
+_FLAG_TYPES = ("Adam", "SGD", "Adagrad", "Rmsprop")
 _ATTR = {"ent": "ent_embeddings", "rel": "rel_embeddings", "norm": "norm_embeddings", "proj": "proj_embeddings",
          "user": "user_embeddings", "item": "item_embeddings", "pref": "pref_embeddings",
          "pref_norm": "pref_norm_embeddings"}
@@ -33,14 +46,34 @@ _ATTR = {"ent": "ent_embeddings", "rel": "rel_embeddings", "norm": "norm_embeddi
 _GATHERED = ("ent", "rel", "norm", "user", "item")
 
 
+def flags_kwargs(FLAGS):
+    """SparseRowOptimizer's keyword arguments for the reference's flags (see SparseRowOptimizer.from_flags)."""
+    t = FLAGS.optimizer_type
+    if t not in _FLAG_TYPES:
+        raise ValueError("optimizer_type must be one of %s" % (_FLAG_TYPES,))
+    momentum = float(FLAGS.momentum) if t in ("SGD", "Rmsprop") else 0.0
+    return dict(optimizer_type=t, lr=float(FLAGS.learning_rate), l2_lambda=float(FLAGS.l2_lambda),
+                clip=float(FLAGS.clipping_max_value), momentum=momentum, rows="all")
+
+
 class SparseRowOptimizer:
     def __init__(self, model, optimizer_type="Adagrad", lr=0.01, l2_lambda=0.0, clip=None,
-                 eps=None, betas=(0.9, 0.999)):
+                 eps=None, betas=(0.9, 0.999), momentum=0.0, alpha=0.99, rows="touched"):
+        """rows: "touched" updates the rows the batch touched (O(batch)); "all" updates every row of the tables the
+        step's loss reaches, as torch.optim's dense step does (O(table)).  momentum: SGD and RMSprop.  alpha: RMSprop.
+        Any setting other than the defaults runs through kgrec_rows_update_ex."""
         if optimizer_type not in _KINDS:
             raise ValueError("optimizer_type must be one of %s" % sorted(_KINDS))
+        if rows not in _ROWS:
+            raise ValueError("rows must be one of %s" % sorted(_ROWS))
         self.model, self.kind, self.lr, self.wd, self.clip = model, _KINDS[optimizer_type], lr, l2_lambda, clip
+        self.momentum, self.alpha, self.rows = float(momentum), float(alpha), rows
+        if self.momentum < 0.0 or (self.momentum and self.kind in (1, 2)):
+            raise ValueError("momentum: >= 0, and for SGD and RMSprop only")
         self.eps = eps if eps is not None else (1e-10 if self.kind == 1 else 1e-8)
         self.betas = betas
+        # the defaults run kgrec_rows_update as before; everything else kgrec_rows_update_ex
+        self.exact = rows != "touched" or self.momentum != 0.0 or self.kind == 3
         self.t = 0
         dev = model._require_cuda()
         self.names = KF.MODEL_TABLES[model.MODEL]
@@ -49,11 +82,36 @@ class SparseRowOptimizer:
         ktup = model.MODEL == _lib.KTUP
         self.marks = {k: torch.zeros(w[k].shape[0], dtype=torch.int32, device=dev)
                       for k in self.names if k in _GATHERED and not (ktup and k in ("rel", "norm"))}
-        self.s1 = {k: torch.zeros_like(w[k]) for k in self.names} if self.kind else {k: None for k in self.names}
-        self.s2 = {k: torch.zeros_like(w[k]) for k in self.names} if self.kind == 2 else {k: None for k in self.names}
+        use_s1 = self.kind != 0 or self.momentum != 0.0         # Adagrad sum, Adam m, RMSprop square_avg, SGD's buffer
+        use_s2 = self.kind == 2 or (self.kind == 3 and self.momentum != 0.0)      # Adam v, RMSprop's momentum buffer
+        self.s1 = {k: torch.zeros_like(w[k]) if use_s1 else None for k in self.names}
+        self.s2 = {k: torch.zeros_like(w[k]) if use_s2 else None for k in self.names}
+        # Adam's step count per table (torch keeps one per parameter and advances it only when the parameter has a
+        # gradient): slot i belongs to self.names[i]
+        self.steps = torch.zeros(len(self.names), dtype=torch.int64, device=dev) if self.exact and self.kind == 2 else None
         self.sqnorm = torch.zeros(1, dtype=torch.float32, device=dev)
         self.reg_loss = torch.zeros(1, dtype=torch.float32, device=dev)
         self._rows_ws = None          # work buffers of the row-factored soft rec step, allocated on first use
+
+    @classmethod
+    def from_flags(cls, model, FLAGS):
+        """What the reference's ModelTrainer.optimizer_reset builds (utils/trainer.py:63-78) from -optimizer_type,
+        -learning_rate, -l2_lambda and -momentum, with the drivers' clip_grad_norm at -clipping_max_value, as an exact
+        (rows="all") optimizer: momentum for SGD and Rmsprop only, torch's default eps / betas / alpha."""
+        return cls(model, **flags_kwargs(FLAGS))
+
+    def reset(self, lr):
+        """The trainer's optimizer_reset (utils/trainer.py:98-102, learning-rate decay): a fresh optimizer at `lr` --
+        the rule's state and Adam's step counts are zeroed in place on the current stream (nothing is reallocated, so
+        captured graphs stay valid)."""
+        if self.kind == 2 and self.steps is None:
+            raise ValueError("reset: Adam restarts its step count only with per-table step counts (rows='all')")
+        for v in list(self.s1.values()) + list(self.s2.values()):
+            if v is not None:
+                v.zero_()
+        if self.steps is not None:
+            self.steps.zero_()
+        self.lr = float(lr)
 
     # -- shared tail of every step: marks -> total norm -> update --------------------------------------
     def _seg(self, ids, table, compact=False, remap=None):
@@ -99,6 +157,10 @@ class SparseRowOptimizer:
             else:
                 _lib.check(lib.kgrec_rows_sqnorm_dev(tab_arr, len(entries), state.ptr, KF._ptr(self.sqnorm), stream))
         sq = KF._ptr(self.sqnorm) if use_clip else None
+        if self.exact:
+            self._update_ex(tables, tab_arr, len(entries), sq, state)
+            KF.count_launches(1 + int(use_clip) + int(self.steps is not None))
+            return
         if state is None:
             _lib.check(lib.kgrec_rows_update(tab_arr, len(entries), self.t, self.kind, self.lr, self.eps, self.betas[0],
                                              self.betas[1], self.t, self.wd, sq, float(self.clip or 0.0), stream))
@@ -106,6 +168,22 @@ class SparseRowOptimizer:
             _lib.check(lib.kgrec_rows_update_dev(tab_arr, len(entries), state.ptr, self.kind, self.eps, self.betas[0],
                                                  self.betas[1], self.wd, sq, float(self.clip or 0.0), stream))
         KF.count_launches(1 + int(use_clip))
+
+    def _update_ex(self, tables, tab_arr, n, sq, state):
+        steps = None
+        if self.steps is not None:          # the call's tables are a run of self.names: its counters are a slice
+            i = self.names.index(tables[0])
+            if tuple(self.names[i:i + n]) != tuple(tables):
+                raise AssertionError("tables of one update must be a run of the optimizer's tables")
+            steps = self.steps.data_ptr() + 8 * i
+        P = _lib.OptParams(kind=self.kind, rows=_ROWS[self.rows], lr=self.lr, eps=self.eps, beta1=self.betas[0],
+                           beta2=self.betas[1], alpha=self.alpha, momentum=self.momentum, weight_decay=self.wd,
+                           max_norm=float(self.clip or 0.0), step_counts=steps)
+        lib = _lib.load()
+        if state is None:
+            _lib.check(lib.kgrec_rows_update_ex(tab_arr, n, self.t, C.byref(P), sq, KF._stream()))
+        else:               # epoch and lr from the device step state
+            _lib.check(lib.kgrec_rows_update_ex_dev(tab_arr, n, state.ptr, C.byref(P), sq, KF._stream()))
 
     def _apply(self, segs, tables, state=None):
         """segs: MarkSeg list of this step's id arrays; tables: names of the tables the step's loss reaches."""

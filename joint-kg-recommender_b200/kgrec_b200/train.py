@@ -9,6 +9,7 @@ One step is the loop of INTEGRATION section 6 on the device:
     kgrec_sample_*_dev        negatives, seed = sample_seed + step
     loss step                 kgrec_corrupt_loss_step (KG) / kgrec_rank_loss_step_dev | kgrec_rec_rows_step_dev (rec)
     kgrec_rows_*_dev          marks, clip norm, SGD / Adagrad / Adam with lr and Adam's t read from the state
+                              (kgrec_rows_update_ex_dev for the optimizer's exact / momentum / RMSprop settings)
 
 Every scalar that changes from step to step is read from the device step state, so a graph of S such steps can be
 replayed as it is.  Epoch boundaries are kept on the host: run() knows from DeviceTrainIterator's rule how many batches
@@ -211,6 +212,7 @@ class GraphedTrainLoop:
         m, opt = self.model, self.opt
         ts = list(m.parameters()) + list(opt.acc.values()) + list(opt.marks.values()) + [opt.sqnorm, opt.reg_loss]
         ts += [v for v in list(opt.s1.values()) + list(opt.s2.values()) if v is not None]
+        ts += [opt.steps] if opt.steps is not None else []
         ts += [self.state.buf, self._status] + [s.cursor for s in self.src.values()]
         ts += [s.sampler._status() for s in self.src.values()]
         return ts
@@ -274,6 +276,13 @@ class GraphedTrainLoop:
         recapture."""
         self.opt.lr = float(lr)
         self.state.set_lr(lr)
+
+    def reset_optimizer(self, lr):
+        """The trainer's optimizer_reset between replays: SparseRowOptimizer.reset(lr) (state and Adam's per-table step
+        counts zeroed in place) and set_lr(lr).  No recapture: the buffers keep their addresses and the step counts are
+        read on the device."""
+        self.opt.reset(lr)
+        self.set_lr(lr)
 
     def check(self):
         """Raise if an id was out of range or a sampler key had no valid negative since the last check (device sync)."""
