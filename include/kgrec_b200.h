@@ -223,9 +223,11 @@ int kgrec_corrupt_loss_bwd(const kgrec_tables* tables, int model,
  * (knowledge_representation.py:197-204): normLoss (loss.py:21-23) over the entity rows of
  * cat[ph, pt, nh, nt] and the relation rows of cat[pr, nr], and for TransH orthogonalLoss
  * (loss.py:18-19) over (rel, norm) rows of cat[pr, nr] -- every row with the multiplicity it has in
- * those lists.  Margin loss and embedding_size <= 128 only.
+ * those lists.  Margin loss and embedding_size <= 128 only; reg_flags other than 0 / 1 is
+ * KGREC_ERR_INVALID, reg_flags 1 with the BPR loss KGREC_ERR_UNSUPPORTED.
  * KGREC_TRANSR is accepted by this entry point as well (embedding_size <= 128, n_neg <= 14,
- * reg_flags 0): the relation's d x d matrix is read twice per GROUP and its gradient
+ * reg_flags 0 or 1; normLoss over the raw ent / rel rows as above, none on proj, as the
+ * reference): the relation's d x d matrix is read twice per GROUP and its gradient
  * (grads->proj, always a dense [n_rel, d*d] accumulate) added once per group; the groups are
  * visited in relation order (a counting sort of pr inside the call) so that a CTA's warps share M_r.
  * workspace: >= kgrec_corrupt_loss_step_workspace_bytes(tables, model, n_pos) bytes. */

@@ -1100,7 +1100,11 @@ k_group_step_h(const GroupArgs G, const float up0, const float* __restrict__ up_
 //   * transposes G through shared memory and computes the entity-row gradients M^T G with lanes owning
 //     16-byte column chunks (coalesced second pass over M), storing the 2 + K slot rows.
 // M is read twice per group instead of twice per triple, the atomics drop by 1 + K.
-template <int NVT, bool MARGIN>
+// REG adds the drivers' normLoss (knowledge_representation.py:197-204) over the RAW rows h, t, c_k and r -- the reference
+// regularises model.ent_embeddings / rel_embeddings, not the projections, and M has no regulariser -- with each row's
+// multiplicity in cat[ph, pt, nh, nt] and cat[pr, nr] (the k_group_step_e / _h definition): the norms come from V in
+// shared memory and from the relation row in registers.
+template <int NVT, bool MARGIN, bool REG>
 __global__ void __launch_bounds__(kThreads, 1)
 k_group_step_r(const GroupArgs G, const float up0, float* __restrict__ pos_scores, float* __restrict__ neg_scores,
                float* __restrict__ group_loss, const kgrec_grads Gr, int64_t* __restrict__ slot_ent,
@@ -1242,9 +1246,40 @@ k_group_step_r(const GroupArgs G, const float up0, float* __restrict__ pos_score
         y[i][1] = gt[i] - g;                                       // G for t
       }
     }
+    // REG: |V_v|^2 per staged row (lane v keeps row v's gradient coefficient for the entity pass), |r|^2 from rr
+    [[maybe_unused]] float creg = 0.f, lreg = 0.f;
+    if (REG) {
+      const float r2 = 2.f * up0;
+      const float n_tail = static_cast<float>(__popc(__ballot_sync(FULL, lane < K && cv >= 0)));
+      float n2 = 0.f;
+#pragma unroll
+      for (int v = 0; v < NVT; ++v) {
+        if (v < nv) {
+          float s = 0.f;
+          if (lane < NC) {
+            const float4 x = Vs[v * NC + lane];
+            s = x.x * x.x + x.y * x.y + x.z * x.z + x.w * x.w;
+          }
+          s = warp_sum(s);
+          if (lane == v) n2 = s;
+        }
+      }
+      float nr2 = 0.f;
+#pragma unroll
+      for (int i = 0; i < 4; ++i) nr2 += rr[i] * rr[i];             // rr is 0 past d
+      nr2 = warp_sum(nr2);
+      // h is listed once as ph and once per tail-replaced negative (nh); t likewise; r once per triple
+      const float m = lane == 0 ? 1.f + n_tail : (lane == 1 ? 1.f + (static_cast<float>(K) - n_tail) : 1.f);
+      creg = lane < nv && n2 > 1.f ? m * r2 : 0.f;
+      const float mr = 1.f + static_cast<float>(K);
+      lreg = warp_sum(lane < nv ? m * fmaxf(n2 - 1.f, 0.f) : 0.f) + mr * fmaxf(nr2 - 1.f, 0.f);
+      const float cr = nr2 > 1.f ? mr * r2 : 0.f;
+#pragma unroll
+      for (int i = 0; i < 4; ++i) gp[i] = fmaf(cr, rr[i], gp[i]);
+    }
     if (lane == 0) {
       pos_scores[j] = sp;
-      group_loss[j] = lsum;
+      group_loss[j] = REG ? lsum + lreg : lsum;
     }
     if (lane < K) neg_scores[static_cast<int64_t>(j) * K + lane] = mys;
     // relation-row gradient
@@ -1292,7 +1327,16 @@ k_group_step_r(const GroupArgs G, const float up0, float* __restrict__ pos_score
     // ---- entity-row gradients M^T G, lane owns column chunk `lane`
     float4 gv[NVT];
 #pragma unroll
-    for (int v = 0; v < NVT; ++v) gv[v] = make_float4(0.f, 0.f, 0.f, 0.f);
+    for (int v = 0; v < NVT; ++v) {
+      gv[v] = make_float4(0.f, 0.f, 0.f, 0.f);
+      if (REG) {                            // the regulariser's 2 m x first, M^T G accumulates onto it
+        const float c = __shfl_sync(FULL, creg, v);
+        if (c != 0.f && lane < NC) {
+          const float4 x = Vs[v * NC + lane];
+          gv[v] = make_float4(c * x.x, c * x.y, c * x.z, c * x.w);
+        }
+      }
+    }
     if (lane < NC) {
       for (int a = 0; a < d; ++a) {
         const float4 mrow = __ldg(reinterpret_cast<const float4*>(M + static_cast<size_t>(a) * d) + lane);
@@ -1345,6 +1389,11 @@ k_group_step_r(const GroupArgs G, const float up0, float* __restrict__ pos_score
 // two fp32-pair FMAs (fma2) per pair of 16-byte operands, no splats; QF = d / 32 full lane-rows, the d - 32 QF rows left
 // (4 at d = 100) in a short (row, lane) pass instead of a quarter-empty fourth accumulator column.  The row pitch is an
 // odd number of 16-byte units: the lane-per-row reads are conflict-free.
+// REG (the normLoss terms, as in k_group_step_r): V is single-buffered and the next tile's rows land in it while dV is
+// computed, so the raw rows are gone by the dV epilogue.  The loss stage, where each warp still reads its group's rows
+// from sV, writes the term 2 m x of every row outside the unit sphere to the row's gradient destination: an atomic add
+// (dense) or a store to the row's slot, whose pointer in sDst is then tagged (bit 0) so that the dV epilogue adds to the
+// slot (red.add) instead of storing.  Two __syncthreads separate the two writes.
 __host__ __device__ inline int run_pitch(int d) { return ((d >> 2) & 1) ? d : d + 4; }
 
 template <int QF, typename Emit>
@@ -1389,7 +1438,7 @@ __device__ __forceinline__ void run_tile_dot(const float* __restrict__ A, const 
   }
 }
 
-template <int QA, int QB, int QF, int RB, bool MARGIN>
+template <int QA, int QB, int QF, int RB, bool MARGIN, bool REG>
 __global__ void __launch_bounds__(kThreads, 1)
 k_run_step_r(const GroupArgs G, const float up0, float* __restrict__ pos_scores, float* __restrict__ neg_scores,
              float* __restrict__ group_loss, const kgrec_grads Gr, int64_t* __restrict__ slot_ent,
@@ -1445,6 +1494,7 @@ k_run_step_r(const GroupArgs G, const float up0, float* __restrict__ pos_scores,
   const int i_end = min(n_pos, (static_cast<int>(blockIdx.x) + 1) * chunk);
   int cur_rel = -1;
   float rr[4] = {0.f, 0.f, 0.f, 0.f};
+  [[maybe_unused]] float nr2 = 0.f;                  // REG: |r|^2 of the current relation
 
   // The tile that starts at group i_from of the order (one warp): its groups -- the leading ones of the chunk's rest that
   // share a relation --, then per tile row the table row to copy from and the place its gradient goes to.
@@ -1526,6 +1576,7 @@ k_run_step_r(const GroupArgs G, const float up0, float* __restrict__ pos_scores,
         const int a = lane + 32 * i;
         rr[i] = a < d ? __ldg(T.rel + static_cast<uint64_t>(rel) * T.ld + a) : 0.f;
       }
+      if (REG) nr2 = warp_sum(rr[0] * rr[0] + rr[1] * rr[1] + rr[2] * rr[2] + rr[3] * rr[3]);
       __syncthreads();
     }
     // ---- Y = V M^T
@@ -1595,6 +1646,45 @@ k_run_step_r(const GroupArgs G, const float up0, float* __restrict__ pos_scores,
           if (a < d) Yc[a] = head ? g : -g;
         }
       }
+      [[maybe_unused]] float lreg = 0.f;
+      if (REG) {
+        const float r2 = 2.f * up0;
+        const float n_tail = static_cast<float>(__popc(__ballot_sync(FULL, lane < K && cv >= 0)));
+        const int n0 = gq * nv;
+        for (int v = 0; v < nv; ++v) {
+          const float* x = sV + (n0 + v) * pitch;
+          float xv[4], s = 0.f;
+#pragma unroll
+          for (int i = 0; i < 4; ++i) {
+            const int a = lane + 32 * i;
+            xv[i] = a < d ? x[a] : 0.f;
+            s += xv[i] * xv[i];
+          }
+          s = warp_sum(s);
+          // h is listed once as ph and once per tail-replaced negative (nh); t likewise
+          const float m = v == 0 ? 1.f + n_tail : (v == 1 ? 1.f + (static_cast<float>(K) - n_tail) : 1.f);
+          lreg += m * fmaxf(s - 1.f, 0.f);
+          if (s > 1.f) {                                           // warp-uniform
+            const float c = m * r2;
+            float* dst = sDst[buf * ROWS + n0 + v];
+#pragma unroll
+            for (int i = 0; i < 4; ++i) {
+              const int a = lane + 32 * i;
+              if (a < d) {
+                if (Gr.mode) atomicAdd(dst + a, c * xv[i]);
+                else dst[a] = c * xv[i];
+              }
+            }
+            __syncwarp();
+            if (!Gr.mode && lane == 0) sDst[buf * ROWS + n0 + v] = reinterpret_cast<float*>(reinterpret_cast<uintptr_t>(dst) | 1u);
+          }
+        }
+        const float mr = 1.f + static_cast<float>(K);                // r once per triple
+        lreg += mr * fmaxf(nr2 - 1.f, 0.f);
+        const float cr = nr2 > 1.f ? mr * r2 : 0.f;
+#pragma unroll
+        for (int i = 0; i < 4; ++i) gp[i] = fmaf(cr, rr[i], gp[i]);
+      }
       const float cp = cpos * up;
 #pragma unroll
       for (int i = 0; i < 4; ++i) {
@@ -1608,7 +1698,7 @@ k_run_step_r(const GroupArgs G, const float up0, float* __restrict__ pos_scores,
           else atomicAdd(Gr.rel + static_cast<uint64_t>(rel) * d + a, gp[i]);
         }
       }
-      if (lane == 0) { pos_scores[j] = sp; group_loss[j] = lsum; }
+      if (lane == 0) { pos_scores[j] = sp; group_loss[j] = REG ? lsum + lreg : lsum; }
       if (lane < K) neg_scores[static_cast<int64_t>(j) * K + lane] = mys;
     }
     if (wid == kWarpsPerCta - 1) plan(buf ^ 1, i0 + ng);          // the next tile's rows, while the other warps finish their groups
@@ -1656,8 +1746,15 @@ k_run_step_r(const GroupArgs G, const float up0, float* __restrict__ pos_scores,
       float* const* dstp = sDst + buf * ROWS + base;
       run_tile_dot<QF>(sG + base * pitch, sMt, d, NC, pitch, lane, [&](int i, int b, float v) {
         if (base + i < rows) {
-          float* dst = dstp[i] + b;
-          if (dense) atomicAdd(dst, v); else __stcs(dst, v);
+          if (REG) {                     // a tagged slot holds the regulariser's term already: add to it (a reduction, not
+                                         // a load + store: nothing waits on it, and the slot is this row's alone)
+            const uintptr_t p = reinterpret_cast<uintptr_t>(dstp[i]);
+            float* dst = reinterpret_cast<float*>(p & ~static_cast<uintptr_t>(1)) + b;
+            if (dense || (p & 1)) atomicAdd(dst, v); else __stcs(dst, v);
+          } else {
+            float* dst = dstp[i] + b;
+            if (dense) atomicAdd(dst, v); else __stcs(dst, v);
+          }
         }
       });
     }
@@ -1895,8 +1992,9 @@ extern "C" int kgrec_corrupt_loss_step(const kgrec_tables* tables, int model, co
     return KGREC_ERR_INVALID;
   }
   if ((slot_ent_ids == nullptr) != (slot_rel_ids == nullptr)) { set_error("slot_ent_ids and slot_rel_ids go together"); return KGREC_ERR_INVALID; }
+  if (reg_flags != 0 && reg_flags != 1) { set_error("reg_flags must be 0 or 1"); return KGREC_ERR_INVALID; }
+  if (reg_flags && loss_kind != KGREC_LOSS_MARGIN) { set_error("fused regularisers go with the margin loss (the KG drivers' loss)"); return KGREC_ERR_UNSUPPORTED; }
   if (pl.fam == FAM_R) {
-    if (reg_flags) { set_error("fused regularisers are built for TransE / TransH"); return KGREC_ERR_UNSUPPORTED; }
     if (pl.nch != 1 || n_neg > 14) { set_error("TransR step kernel: embedding_size <= 128 and at most 14 negatives per positive"); return KGREC_ERR_UNSUPPORTED; }
     if (n_pos == 0) return KGREC_OK;
     const GroupArgs GA{*tables, ph, pt, pr, idx_bytes == 8, corrupt, LossCfg{loss_kind, margin_or_target, n_neg, n_pos, batch_pos}, 1.f};
@@ -1930,7 +2028,8 @@ extern "C" int kgrec_corrupt_loss_step(const kgrec_tables* tables, int model, co
       const int grid = static_cast<int>(want < sm_count() ? want : sm_count());
 #define CALL_RUN(QAV, QBV, QFV, RBV)                                                                                     \
   {                                                                                                                      \
-    auto kern = mg ? k_run_step_r<QAV, QBV, QFV, RBV, true> : k_run_step_r<QAV, QBV, QFV, RBV, false>;                   \
+    auto kern = reg_flags ? k_run_step_r<QAV, QBV, QFV, RBV, true, true>                                                 \
+                          : (mg ? k_run_step_r<QAV, QBV, QFV, RBV, true, false> : k_run_step_r<QAV, QBV, QFV, RBV, false, false>); \
     KGREC_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));       \
     kern<<<grid, kThreads, smem, s2>>>(GA, grad_loss, pos_scores, neg_scores, gl, *grads, slot_ent_ids, slot_rel_ids, status, order); \
   }
@@ -1943,15 +2042,15 @@ extern "C" int kgrec_corrupt_loss_step(const kgrec_tables* tables, int model, co
     const int grid_r = static_cast<int>(want < sm_count() ? want : sm_count());          // one resident CTA per SM
     const int nvt = n_neg <= 2 ? 4 : (n_neg <= 10 ? 12 : 16);
     const size_t smem = static_cast<size_t>(kWarpsPerCta) * (static_cast<size_t>(nvt) * (tables->dim / 4) + static_cast<size_t>(tables->dim) * (nvt / 4)) * 16;
-#define CALL_R(NVTV, MV)                                                                                             \
+#define CALL_R(NVTV, MV, RV)                                                                                         \
   {                                                                                                                  \
-    auto kern = k_group_step_r<NVTV, MV>;                                                                            \
+    auto kern = k_group_step_r<NVTV, MV, RV>;                                                                        \
     KGREC_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));   \
     kern<<<grid_r, kThreads, smem, s2>>>(GA, grad_loss, pos_scores, neg_scores, gl, *grads, slot_ent_ids, slot_rel_ids, status, order); \
   }
-    if (nvt == 4) { if (mg) CALL_R(4, true) else CALL_R(4, false) }
-    else if (nvt == 12) { if (mg) CALL_R(12, true) else CALL_R(12, false) }
-    else { if (mg) CALL_R(16, true) else CALL_R(16, false) }
+    if (nvt == 4) { if (reg_flags) CALL_R(4, true, true) else if (mg) CALL_R(4, true, false) else CALL_R(4, false, false) }
+    else if (nvt == 12) { if (reg_flags) CALL_R(12, true, true) else if (mg) CALL_R(12, true, false) else CALL_R(12, false, false) }
+    else { if (reg_flags) CALL_R(16, true, true) else if (mg) CALL_R(16, true, false) else CALL_R(16, false, false) }
 #undef CALL_R
     }
     KGREC_CUDA_OK(cudaGetLastError());
@@ -1965,8 +2064,6 @@ extern "C" int kgrec_corrupt_loss_step(const kgrec_tables* tables, int model, co
                     l2_keep_fraction(static_cast<double>(tables->n_ent) * tables->ld * sizeof(float))};
   float* group_loss = static_cast<float*>(workspace);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  if (reg_flags != 0 && reg_flags != 1) { set_error("reg_flags must be 0 or 1"); return KGREC_ERR_INVALID; }
-  if (reg_flags && loss_kind != KGREC_LOSS_MARGIN) { set_error("fused regularisers go with the margin loss (the KG drivers' loss)"); return KGREC_ERR_UNSUPPORTED; }
   // KGREC_GROUP_STEP (A/B runs, tests): 0 = the general kernel for every shape; n = no row prefetch;
   // 3 (TransE) / 2 (TransH) = fewer CTAs per SM, no prefetch
   const char* env = group_step_env();

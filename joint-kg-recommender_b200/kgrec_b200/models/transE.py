@@ -52,7 +52,8 @@ class KGModelBase(KGRecModule):
         upstream -- the case in all the reference drivers, which call backward() on the loss.
         reg=True: the loss of knowledge_representation.py:189-204 in full -- the ranking loss plus
         normLoss over the gathered entity / relation rows (and orthogonalLoss for TransH) -- values
-        and gradients from the same kernel pass."""
+        and gradients from the same kernel pass.  For TransR the norms are those of the raw ent / rel
+        rows, not the projected ones, and proj has no regulariser, as in the reference."""
         return self._loss_step_corrupt(self.MODEL, pos, corrupt, loss, margin, batch_pos, grad_loss, reg)
 
     def graphed_loss_step(self, n_pos, n_neg, margin=1.0, loss="margin", batch_pos=None, grad_loss=1.0, reg=False):

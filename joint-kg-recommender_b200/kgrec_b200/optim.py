@@ -201,7 +201,8 @@ class SparseRowOptimizer:
     def step_corrupt(self, pos, corrupt, margin=1.0, loss="margin", batch_pos=None, reg=False, grad_loss=1.0, state=None):
         """One training step on positives (h, t, r) and group-compact negatives; returns the
         per-batch losses (device tensor; nothing synchronises).  reg=True adds the KG drivers'
-        normLoss / orthogonalLoss regularisers inside the same kernel (kgrec_corrupt_loss_step).
+        normLoss / orthogonalLoss regularisers inside the same kernel (kgrec_corrupt_loss_step), for
+        TransE / TransH / TransR alike (TransR: normLoss of the raw ent / rel rows; proj has none).
         KTUP: the joint model's KG branch (TransH on ent / rel / norm), grad_loss = kg_lambda.
         state (kgrec_b200.train.StepState, advanced for this step): the optimizer reads its epoch mark, learning rate
         and step count on the device (the `_dev` entry points) -- the step a GraphedTrainLoop captures."""
