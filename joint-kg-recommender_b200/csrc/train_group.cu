@@ -13,7 +13,6 @@
 //
 // Reference arithmetic: transE.py:51-63, transH.py:58-71 (+ utils/misc.py:18-19),
 // utils/loss.py:8-16, 29-31; CPU restatement: oracle/kg_oracle.py.
-#include <cstdlib>
 #include "train_dev.cuh"
 
 namespace kgrec {
@@ -91,19 +90,33 @@ __device__ __forceinline__ uint32_t group_idx(const void* p, int j, int is64, in
   return static_cast<uint32_t>(v);
 }
 
-template <int FAM, int NCH, bool L1>
-__global__ void __launch_bounds__(kThreads)
-k_group_fwd(const GroupArgs G, float* __restrict__ pos_scores, float* __restrict__ neg_scores,
-            float* __restrict__ group_loss, int32_t* status) {
+// ---- forward + loss + backward in one pass ------------------------------------------------
+// d(sum of the per-batch losses)/d(tables) together with the scores and the losses: every
+// reference driver calls backward() on the loss itself (knowledge_representation.py:207), so
+// the upstream of each loss term is known (`up`, times 1/(cnt K) for the BPR mean) while the
+// group is still in registers: one gather of (3 + K) rows, (3 + K) gradient rows written.
+// The general form: any d the row layout takes, any K, 64-bit slot offsets.  Two more modes:
+//   FWD: kgrec_corrupt_loss_fwd -- scores and per-group losses, no gradient;
+//   BWD: its autograd backward -- the coefficients come from the SAVED scores, the upstream is
+//        up0 * up_dev[batch], the positive's contribution seeds the shared-row accumulators ahead
+//        of the negatives (so it rounds differently from STEP, which adds it last), and nothing but
+//        the gradients is written (the host passes no status word).
+// slots (Gr.mode 0): ent [n_pos * (2 + K), d] per group: h, t, c_1 .. c_K ; rel / norm [n_pos, d]
+template <int FAM, int NCH, bool L1, bool BWD = false, bool FWD = false>
+__global__ void __launch_bounds__(kThreads, (!BWD && !FWD && NCH == 1 && FAM == FAM_E) ? 4 : 1)
+k_group_step(const GroupArgs G, const float up0, float* __restrict__ pos_scores, float* __restrict__ neg_scores,
+             float* __restrict__ group_loss, const kgrec_grads Gr, int32_t* status, const float* __restrict__ up_dev) {
   using R = Row<NCH, true>;
   constexpr int NE = NCH * 4;
-  const kgrec_tables& T = G.T;
-  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-  const int K = G.L.n_neg, d = T.dim;
   constexpr int l1 = L1 ? 1 : 0;
-  const int n_pos = static_cast<int>(G.L.n_pos);
+  const kgrec_tables& T = G.T;
+  const LossCfg& L = G.L;
+  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+  const int K = L.n_neg, d = T.dim;
+  const int n_pos = static_cast<int>(L.n_pos);
   const uint32_t n_ent = static_cast<uint32_t>(T.n_ent), ld = static_cast<uint32_t>(T.ld);
-  const uint64_t pol_keep = policy_evict_last(G.keep);
+  const int bp = static_cast<int>(L.batch_pos < 0x7fffffff ? L.batch_pos : 0x7fffffff);
+  const uint64_t pol_keep = policy_evict_last(G.keep), pol_stream = policy_evict_first();
   for (int j = blockIdx.x * kWarpsPerCta + wid; j < n_pos; j += gridDim.x * kWarpsPerCta) {
     const int32_t* cj = G.corrupt + static_cast<int64_t>(j) * K;
     int32_t c = K > 0 ? __ldg(cj) : 0;                       // first negative's id, in flight with the rows
@@ -112,80 +125,21 @@ k_group_fwd(const GroupArgs G, float* __restrict__ pos_scores, float* __restrict
     const uint32_t ir = group_idx(G.pr, j, G.is64, T.n_rel, status);
     GroupPos<FAM, NCH> P;
     P.load(T, ih, it, ir, lane, pol_keep);
-    const float sp = dist_sum(P.epos, l1);
-    float lsum = 0.f;
-    // software pipeline over the negatives: row k+1 is requested before row k is consumed
-    float x[NE], xn[NE];
-    bool head = c < 0;
-    uint32_t id = static_cast<uint32_t>(head ? ~c : c);
-    if (id >= n_ent) { if (status) *status = 1; id = 0; }
-    if (K > 0) R::load_hint(x, row_ptr(T.ent, id, ld), d, lane, pol_keep);
-    for (int k = 0; k < K; ++k) {
-      bool headn = false;
-      if (k + 1 < K) {
-        const int32_t cn = __ldg(cj + k + 1);
-        headn = cn < 0;
-        uint32_t idn = static_cast<uint32_t>(headn ? ~cn : cn);
-        if (idn >= n_ent) { if (status) *status = 1; idn = 0; }
-        R::load_hint(xn, row_ptr(T.ent, idn, ld), d, lane, pol_keep);
-      }
-      float ax = 0.f;
-      if (FAM == FAM_H) ax = warp_sum(R::dot(x, P.w));
-      float e[NE];
-      P.residual(x, head, ax, e);
-      const float sn = dist_sum(e, l1);
-      if (lane == 0) neg_scores[static_cast<int64_t>(j) * K + k] = sn;
-      lsum += loss_term(G.L, sp, sn);
-      head = headn;
-#pragma unroll
-      for (int i = 0; i < NE; ++i) x[i] = xn[i];
-    }
-    if (lane == 0) {
-      pos_scores[j] = sp;
-      group_loss[j] = lsum;
-    }
-  }
-}
-
-// slots (mode 0): ent [n_pos * (2 + K), d] per group: h, t, c_1 .. c_K ; rel / norm [n_pos, d]
-template <int FAM, int NCH, bool L1>
-__global__ void __launch_bounds__(kThreads)
-k_group_bwd(const GroupArgs G, const float* __restrict__ pos_scores, const float* __restrict__ neg_scores,
-            const float grad_loss, const float* __restrict__ grad_loss_dev, const kgrec_grads Gr) {
-  using R = Row<NCH, true>;
-  constexpr int NE = NCH * 4;
-  const kgrec_tables& T = G.T;
-  const LossCfg& L = G.L;
-  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-  const int K = L.n_neg, d = T.dim;
-  constexpr int l1 = L1 ? 1 : 0;
-  const int n_pos = static_cast<int>(L.n_pos);
-  const uint32_t n_ent = static_cast<uint32_t>(T.n_ent), ld = static_cast<uint32_t>(T.ld);
-  const int bp = static_cast<int>(L.batch_pos < 0x7fffffff ? L.batch_pos : 0x7fffffff);
-  const uint64_t pol_keep = policy_evict_last(G.keep), pol_stream = policy_evict_first();
-  for (int j = blockIdx.x * kWarpsPerCta + wid; j < n_pos; j += gridDim.x * kWarpsPerCta) {
-    const int32_t* cj = G.corrupt + static_cast<int64_t>(j) * K;
-    const float* snj = neg_scores + static_cast<int64_t>(j) * K;
-    int32_t c = K > 0 ? __ldg(cj) : 0;
-    const uint32_t ih = group_idx(G.ph, j, G.is64, T.n_ent, nullptr);
-    const uint32_t it = group_idx(G.pt, j, G.is64, T.n_ent, nullptr);
-    const uint32_t ir = group_idx(G.pr, j, G.is64, T.n_rel, nullptr);
-    GroupPos<FAM, NCH> P;
-    P.load(T, ih, it, ir, lane, pol_keep);
-    // upstream of this group: dLoss/d(loss term) = grad_loss * grad_loss_dev[batch] * (1 | 1/(cnt K))
-    const int b = j / bp;
-    float up = grad_loss * (grad_loss_dev ? __ldg(grad_loss_dev + b) : 1.f);
+    float up = up0;
+    if (BWD && up_dev) up *= __ldg(up_dev + j / bp);
     if (L.kind == KGREC_LOSS_BPR) {
-      const int cnt = min(bp, n_pos - b * bp);
-      up /= static_cast<float>(cnt) * static_cast<float>(K);
+      const int b = j / bp;
+      up /= static_cast<float>(min(bp, n_pos - b * bp)) * static_cast<float>(K);
     }
-    const float sp = __ldg(pos_scores + j);
-    float cpos = 0.f;
-    for (int k = lane; k < K; k += 32) cpos += loss_dpos(L, sp, __ldg(snj + k));
-    cpos = warp_sum(cpos) * up;
-
+    const float* snj = neg_scores + static_cast<int64_t>(j) * K;
+    const float sp = BWD ? __ldg(pos_scores + j) : dist_sum(P.epos, l1);
+    float lsum = 0.f, cpos = 0.f;
     float gh[NE], gt[NE], gr[NE], gw[NE];
-    {
+#pragma unroll
+    for (int i = 0; i < NE; ++i) { gh[i] = 0.f; gt[i] = 0.f; gr[i] = 0.f; gw[i] = 0.f; }
+    if (BWD) {   // the positive's own contribution first, with the coefficient summed over its negatives
+      for (int k = lane; k < K; k += 32) cpos += loss_dpos(L, sp, __ldg(snj + k));
+      cpos = warp_sum(cpos) * up;
       float eps[NE];
 #pragma unroll
       for (int i = 0; i < NE; ++i) eps[i] = cpos * ddist_term(P.epos[i], l1);
@@ -198,112 +152,11 @@ k_group_bwd(const GroupArgs G, const float* __restrict__ pos_scores, const float
         gh[i] = gx;
         gt[i] = -gx;
         gr[i] = eps[i];
-        gw[i] = (FAM == FAM_H) ? -(ew * (P.h[i] - P.t[i]) + xw * eps[i]) : 0.f;
+        if (FAM == FAM_H) gw[i] = -(ew * (P.h[i] - P.t[i]) + xw * eps[i]);
       }
     }
     const int64_t slot0 = static_cast<int64_t>(j) * (2 + K);
-    float x[NE], xn[NE];
-    bool head = c < 0;
-    uint32_t id = static_cast<uint32_t>(head ? ~c : c);
-    if (id >= n_ent) id = 0;
-    if (K > 0) R::load_hint(x, row_ptr(T.ent, id, ld), d, lane, pol_keep);
-    for (int k = 0; k < K; ++k) {
-      bool headn = false;
-      uint32_t idn = 0;
-      if (k + 1 < K) {
-        const int32_t cn = __ldg(cj + k + 1);
-        headn = cn < 0;
-        idn = static_cast<uint32_t>(headn ? ~cn : cn);
-        if (idn >= n_ent) idn = 0;
-        R::load_hint(xn, row_ptr(T.ent, idn, ld), d, lane, pol_keep);
-      }
-      const float ck = -loss_dpos(L, sp, __ldg(snj + k)) * up;     // dLoss/d(neg score)
-      float gc[NE];
-      if (ck != 0.f) {                                             // warp-uniform: inactive hinges cost nothing
-        float ax = 0.f;
-        if (FAM == FAM_H) ax = warp_sum(R::dot(x, P.w));
-        float e[NE], eps[NE];
-        P.residual(x, head, ax, e);
-#pragma unroll
-        for (int i = 0; i < NE; ++i) eps[i] = ck * ddist_term(e[i], l1);
-        float ew = 0.f;
-        if (FAM == FAM_H) ew = warp_sum(R::dot(eps, P.w));
-        const float xw = head ? ax - P.b : P.a - ax;               // (h' - t).w or (h - t').w
-#pragma unroll
-        for (int i = 0; i < NE; ++i) {
-          const float gx = (FAM == FAM_H) ? eps[i] - ew * P.w[i] : eps[i];
-          gr[i] += eps[i];
-          if (head) { gc[i] = gx; gt[i] -= gx; }
-          else { gc[i] = -gx; gh[i] += gx; }
-          if (FAM == FAM_H) {
-            const float xd = head ? x[i] - P.t[i] : P.h[i] - x[i];
-            gw[i] -= ew * xd + xw * eps[i];
-          }
-        }
-      } else {
-#pragma unroll
-        for (int i = 0; i < NE; ++i) gc[i] = 0.f;
-      }
-      if (Gr.mode == 0) R::store_hint(Gr.ent + (slot0 + 2 + k) * d, gc, d, lane, pol_stream);
-      else if (ck != 0.f) R::red_add(Gr.ent + static_cast<uint64_t>(id) * d, gc, d, lane);
-      head = headn;
-      id = idn;
-#pragma unroll
-      for (int i = 0; i < NE; ++i) x[i] = xn[i];
-    }
-    if (Gr.mode == 0) {
-      R::store_hint(Gr.ent + slot0 * d, gh, d, lane, pol_stream);
-      R::store_hint(Gr.ent + (slot0 + 1) * d, gt, d, lane, pol_stream);
-      R::store_hint(Gr.rel + static_cast<int64_t>(j) * d, gr, d, lane, pol_stream);
-      if (FAM == FAM_H) R::store_hint(Gr.norm + static_cast<int64_t>(j) * d, gw, d, lane, pol_stream);
-    } else {
-      R::red_add(Gr.ent + static_cast<uint64_t>(ih) * d, gh, d, lane);
-      R::red_add(Gr.ent + static_cast<uint64_t>(it) * d, gt, d, lane);
-      R::red_add(Gr.rel + static_cast<uint64_t>(ir) * d, gr, d, lane);
-      if (FAM == FAM_H) R::red_add(Gr.norm + static_cast<uint64_t>(ir) * d, gw, d, lane);
-    }
-  }
-}
-
-// ---- forward + loss + backward in one pass ------------------------------------------------
-// d(sum of the per-batch losses)/d(tables) together with the scores and the losses: every
-// reference driver calls backward() on the loss itself (knowledge_representation.py:207), so
-// the upstream of each loss term is known (`up`, times 1/(cnt K) for the BPR mean) while the
-// group is still in registers: one gather of (3 + K) rows, (3 + K) gradient rows written.
-template <int FAM, int NCH, bool L1>
-__global__ void __launch_bounds__(kThreads, (NCH == 1 && FAM == FAM_E) ? 4 : 1)
-k_group_step(const GroupArgs G, const float up0, float* __restrict__ pos_scores, float* __restrict__ neg_scores,
-             float* __restrict__ group_loss, const kgrec_grads Gr, int32_t* status) {
-  using R = Row<NCH, true>;
-  constexpr int NE = NCH * 4;
-  constexpr int l1 = L1 ? 1 : 0;
-  const kgrec_tables& T = G.T;
-  const LossCfg& L = G.L;
-  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-  const int K = L.n_neg, d = T.dim;
-  const int n_pos = static_cast<int>(L.n_pos);
-  const uint32_t n_ent = static_cast<uint32_t>(T.n_ent), ld = static_cast<uint32_t>(T.ld);
-  const int bp = static_cast<int>(L.batch_pos < 0x7fffffff ? L.batch_pos : 0x7fffffff);
-  const uint64_t pol_keep = policy_evict_last(G.keep), pol_stream = policy_evict_first();
-  for (int j = blockIdx.x * kWarpsPerCta + wid; j < n_pos; j += gridDim.x * kWarpsPerCta) {
-    const int32_t* cj = G.corrupt + static_cast<int64_t>(j) * K;
-    int32_t c = K > 0 ? __ldg(cj) : 0;
-    const uint32_t ih = group_idx(G.ph, j, G.is64, T.n_ent, status);
-    const uint32_t it = group_idx(G.pt, j, G.is64, T.n_ent, status);
-    const uint32_t ir = group_idx(G.pr, j, G.is64, T.n_rel, status);
-    GroupPos<FAM, NCH> P;
-    P.load(T, ih, it, ir, lane, pol_keep);
-    float up = up0;
-    if (L.kind == KGREC_LOSS_BPR) {
-      const int b = j / bp;
-      up /= static_cast<float>(min(bp, n_pos - b * bp)) * static_cast<float>(K);
-    }
-    const float sp = dist_sum(P.epos, l1);
-    float lsum = 0.f, cpos = 0.f;
-    float gh[NE], gt[NE], gr[NE], gw[NE];
-#pragma unroll
-    for (int i = 0; i < NE; ++i) { gh[i] = 0.f; gt[i] = 0.f; gr[i] = 0.f; gw[i] = 0.f; }
-    const int64_t slot0 = static_cast<int64_t>(j) * (2 + K);
+    // software pipeline over the negatives: row k+1 is requested before row k is consumed
     float x[NE], xn[NE];
     bool head = c < 0;
     uint32_t id = static_cast<uint32_t>(head ? ~c : c);
@@ -320,46 +173,57 @@ k_group_step(const GroupArgs G, const float up0, float* __restrict__ pos_scores,
         R::load_hint(xn, row_ptr(T.ent, idn, ld), d, lane, pol_keep);
       }
       float ax = 0.f;
-      if (FAM == FAM_H) ax = warp_sum(R::dot(x, P.w));
       float e[NE];
-      P.residual(x, head, ax, e);
-      const float sn = dist_sum(e, l1);
-      if (lane == 0) neg_scores[static_cast<int64_t>(j) * K + k] = sn;
-      lsum += loss_term(L, sp, sn);
-      const float dp = loss_dpos(L, sp, sn);
-      cpos += dp;
-      const float ck = -dp * up;
-      float gc[NE];
-      if (ck != 0.f) {                     // warp-uniform: an inactive hinge has no gradient
-        float eps[NE];
-#pragma unroll
-        for (int i = 0; i < NE; ++i) eps[i] = ck * ddist_term(e[i], l1);
-        float ew = 0.f;
-        if (FAM == FAM_H) ew = warp_sum(R::dot(eps, P.w));
-        const float xw = head ? ax - P.b : P.a - ax;
-#pragma unroll
-        for (int i = 0; i < NE; ++i) {
-          const float gx = (FAM == FAM_H) ? eps[i] - ew * P.w[i] : eps[i];
-          gr[i] += eps[i];
-          if (head) { gc[i] = gx; gt[i] -= gx; }
-          else { gc[i] = -gx; gh[i] += gx; }
-          if (FAM == FAM_H) {
-            const float xd = head ? x[i] - P.t[i] : P.h[i] - x[i];
-            gw[i] -= ew * xd + xw * eps[i];
-          }
-        }
+      float ck;                            // dLoss/d(neg score), times -1
+      if (BWD) {
+        ck = -loss_dpos(L, sp, __ldg(snj + k)) * up;
       } else {
-#pragma unroll
-        for (int i = 0; i < NE; ++i) gc[i] = 0.f;
+        if (FAM == FAM_H) ax = warp_sum(R::dot(x, P.w));
+        P.residual(x, head, ax, e);
+        const float sn = dist_sum(e, l1);
+        if (lane == 0) neg_scores[static_cast<int64_t>(j) * K + k] = sn;
+        lsum += loss_term(L, sp, sn);
+        const float dp = loss_dpos(L, sp, sn);
+        cpos += dp;
+        ck = -dp * up;
       }
-      if (Gr.mode == 0) R::store_hint(Gr.ent + (slot0 + 2 + k) * d, gc, d, lane, pol_stream);
-      else if (ck != 0.f) R::red_add(Gr.ent + static_cast<uint64_t>(id) * d, gc, d, lane);
+      if (!FWD) {
+        float gc[NE];
+        if (ck != 0.f) {                     // warp-uniform: an inactive hinge has no gradient
+          if (BWD) {
+            if (FAM == FAM_H) ax = warp_sum(R::dot(x, P.w));
+            P.residual(x, head, ax, e);
+          }
+          float eps[NE];
+#pragma unroll
+          for (int i = 0; i < NE; ++i) eps[i] = ck * ddist_term(e[i], l1);
+          float ew = 0.f;
+          if (FAM == FAM_H) ew = warp_sum(R::dot(eps, P.w));
+          const float xw = head ? ax - P.b : P.a - ax;               // (h' - t).w or (h - t').w
+#pragma unroll
+          for (int i = 0; i < NE; ++i) {
+            const float gx = (FAM == FAM_H) ? eps[i] - ew * P.w[i] : eps[i];
+            gr[i] += eps[i];
+            if (head) { gc[i] = gx; gt[i] -= gx; }
+            else { gc[i] = -gx; gh[i] += gx; }
+            if (FAM == FAM_H) {
+              const float xd = head ? x[i] - P.t[i] : P.h[i] - x[i];
+              gw[i] -= ew * xd + xw * eps[i];
+            }
+          }
+        } else {
+#pragma unroll
+          for (int i = 0; i < NE; ++i) gc[i] = 0.f;
+        }
+        if (Gr.mode == 0) R::store_hint(Gr.ent + (slot0 + 2 + k) * d, gc, d, lane, pol_stream);
+        else if (ck != 0.f) R::red_add(Gr.ent + static_cast<uint64_t>(id) * d, gc, d, lane);
+      }
       head = headn;
       id = idn;
 #pragma unroll
       for (int i = 0; i < NE; ++i) x[i] = xn[i];
     }
-    {   // the positive's own contribution, with the coefficient summed over its negatives
+    if (!FWD && !BWD) {   // the positive's own contribution last, with the coefficient summed over its negatives
       const float cp = cpos * up;
       float eps[NE];
 #pragma unroll
@@ -376,20 +240,22 @@ k_group_step(const GroupArgs G, const float up0, float* __restrict__ pos_scores,
         if (FAM == FAM_H) gw[i] -= ew * (P.h[i] - P.t[i]) + xw * eps[i];
       }
     }
-    if (lane == 0) {
+    if (!BWD && lane == 0) {
       pos_scores[j] = sp;
       group_loss[j] = lsum;
     }
-    if (Gr.mode == 0) {
-      R::store_hint(Gr.ent + slot0 * d, gh, d, lane, pol_stream);
-      R::store_hint(Gr.ent + (slot0 + 1) * d, gt, d, lane, pol_stream);
-      R::store_hint(Gr.rel + static_cast<int64_t>(j) * d, gr, d, lane, pol_stream);
-      if (FAM == FAM_H) R::store_hint(Gr.norm + static_cast<int64_t>(j) * d, gw, d, lane, pol_stream);
-    } else {
-      R::red_add(Gr.ent + static_cast<uint64_t>(ih) * d, gh, d, lane);
-      R::red_add(Gr.ent + static_cast<uint64_t>(it) * d, gt, d, lane);
-      R::red_add(Gr.rel + static_cast<uint64_t>(ir) * d, gr, d, lane);
-      if (FAM == FAM_H) R::red_add(Gr.norm + static_cast<uint64_t>(ir) * d, gw, d, lane);
+    if (!FWD) {
+      if (Gr.mode == 0) {
+        R::store_hint(Gr.ent + slot0 * d, gh, d, lane, pol_stream);
+        R::store_hint(Gr.ent + (slot0 + 1) * d, gt, d, lane, pol_stream);
+        R::store_hint(Gr.rel + static_cast<int64_t>(j) * d, gr, d, lane, pol_stream);
+        if (FAM == FAM_H) R::store_hint(Gr.norm + static_cast<int64_t>(j) * d, gw, d, lane, pol_stream);
+      } else {
+        R::red_add(Gr.ent + static_cast<uint64_t>(ih) * d, gh, d, lane);
+        R::red_add(Gr.ent + static_cast<uint64_t>(it) * d, gt, d, lane);
+        R::red_add(Gr.rel + static_cast<uint64_t>(ir) * d, gr, d, lane);
+        if (FAM == FAM_H) R::red_add(Gr.norm + static_cast<uint64_t>(ir) * d, gw, d, lane);
+      }
     }
   }
 }
@@ -409,8 +275,8 @@ k_group_step(const GroupArgs G, const float up0, float* __restrict__ pos_scores,
 //     load held one per lane (and the positive's three ids one load in lanes 0-2), fetched a whole
 //     group ahead and handed out by shuffles, so the request for row k+1 leaves as soon as row k's
 //     arithmetic starts (with per-negative id loads the row request waits a full L2 round trip).
-template <bool L1, bool DENSE, bool MARGIN, int MINB, bool PF, bool REG, bool BWD, bool FWD = false>
-__global__ void __launch_bounds__(kThreads, MINB)
+template <bool L1, bool DENSE, bool MARGIN, bool REG, bool BWD, bool FWD>
+__global__ void __launch_bounds__(kThreads, 4)
 k_group_step_e(const GroupArgs G, const float up0, const float* __restrict__ up_dev, float* __restrict__ pos_scores,
                float* __restrict__ neg_scores, float* __restrict__ group_loss, const kgrec_grads Gr,
                int64_t* __restrict__ slot_ent, int64_t* __restrict__ slot_rel, int32_t* status) {
@@ -478,7 +344,7 @@ k_group_step_e(const GroupArgs G, const float up0, const float* __restrict__ up_
       r = ldg_f4_hint(row(rel_b, ir), pol_keep);
       xa = ldg_f4_hint(row(ent_b, ida), pol_keep);
     }
-    if (PF && lane >= 2 && lane < K) {     // lane l holds the id of negative l: it pulls that row's lines towards the SM
+    if (lane >= 2 && lane < K) {     // lane l holds the id of negative l: it pulls that row's lines towards the SM
       const uint32_t pid = static_cast<uint32_t>(cv < 0 ? ~cv : cv);
       if (pid < n_ent) {
         const char* pr = reinterpret_cast<const char*>(T.ent) + static_cast<uint64_t>(pid) * ld4;
@@ -856,8 +722,8 @@ k_group_step_e_tma(const GroupArgs G, const float up0, float* __restrict__ pos_s
 //   g_h = E_h - (E_h.w) w,  g_t = E_t - (E_t.w) w,  g_r = accT - accH + eps_p,
 //   g_w -= (E_h.w) h + (h.w) E_h + (E_t.w) t + (t.w) E_t.
 // The two reductions a negative needs after its residual (the score and g.w) share one shuffle tree.
-template <bool L1, bool DENSE, bool MARGIN, int MINB, bool PF, bool REG, bool BWD, bool FWD = false>
-__global__ void __launch_bounds__(kThreads, MINB)
+template <bool L1, bool DENSE, bool MARGIN, bool REG, bool BWD, bool FWD>
+__global__ void __launch_bounds__(kThreads, 3)
 k_group_step_h(const GroupArgs G, const float up0, const float* __restrict__ up_dev, float* __restrict__ pos_scores,
                float* __restrict__ neg_scores, float* __restrict__ group_loss, const kgrec_grads Gr,
                int64_t* __restrict__ slot_ent, int64_t* __restrict__ slot_rel, int32_t* status) {
@@ -927,7 +793,7 @@ k_group_step_h(const GroupArgs G, const float up0, const float* __restrict__ up_
       w = ldg_f4_hint(row(nrm_b, ir), pol_keep);
       xa = ldg_f4_hint(row(ent_b, ida), pol_keep);
     }
-    if (PF && lane >= 2 && lane < K) {     // lane l holds the id of negative l: it pulls that row's lines towards the SM
+    if (lane >= 2 && lane < K) {     // lane l holds the id of negative l: it pulls that row's lines towards the SM
       const uint32_t pid = static_cast<uint32_t>(cv < 0 ? ~cv : cv);
       if (pid < n_ent) {
         const char* pr = reinterpret_cast<const char*>(T.ent) + static_cast<uint64_t>(pid) * ld4;
@@ -1130,7 +996,7 @@ k_group_step_r(const GroupArgs G, const float up0, float* __restrict__ pos_score
   const int i_end = min(n_pos, (static_cast<int>(blockIdx.x) + 1) * chunk);
 
   for (int i = blockIdx.x * chunk + wid; i < i_end; i += kWarpsPerCta) {
-    const int j = order ? __ldg(order + i) : i;
+    const int j = __ldg(order + i);
     const int32_t cv = lane < K ? __ldg(G.corrupt + static_cast<int64_t>(j) * K + lane) : 0;
     const int64_t pv = lane < 3 ? load_idx(pcol, j, G.is64) : 0;
     const int64_t vh = __shfl_sync(FULL, pv, 0), vt = __shfl_sync(FULL, pv, 1), vr = __shfl_sync(FULL, pv, 2);
@@ -1503,7 +1369,7 @@ k_run_step_r(const GroupArgs G, const float up0, float* __restrict__ pos_scores,
     int j = -1;
     int64_t r = -1;
     if (lane < GC && i_from + lane < i_end) {
-      j = order ? __ldg(order + i_from + lane) : i_from + lane;
+      j = __ldg(order + i_from + lane);
       r = load_idx(G.pr, j, G.is64);
       if (static_cast<uint64_t>(r) >= static_cast<uint64_t>(T.n_rel)) { bad = true; r = 0; }
     }
@@ -1824,12 +1690,6 @@ k_rel_scatter(const void* pr, const int is64, const int n_pos, const int64_t n_r
 
 int make_plan(const kgrec_tables* T, int model, Plan* pl);
 
-// KGREC_GROUP_STEP is an A/B / test switch: read once, not on every call of the hot path.
-static const char* group_step_env() {
-  static const char* cached = [] { const char* e = getenv("KGREC_GROUP_STEP"); return e ? e : ""; }();
-  return cached[0] ? cached : nullptr;
-}
-
 // The TMA-staged TransE step kernel runs 16 warps per CTA with 2 stages per warp; it is picked for slot gradients when
 // that ring fits one CTA's shared memory.  Warps x stages measured with the current loop on an H100 80GB HBM3 (400 W)
 // at bench.py's shape (d = 100, K = 10, 262 144 groups), ms per launch at |E| = 10k / 100k (tools/step_e_floor.py):
@@ -1859,16 +1719,88 @@ static int group_check(const kgrec_tables* T, int model, Plan* pl, const void* p
   return KGREC_OK;
 }
 
+static GroupArgs group_args(const kgrec_tables* T, const void* ph, const void* pt, const void* pr, int idx_bytes,
+                            int64_t n_pos, const int32_t* corrupt, int32_t n_neg, int64_t batch_pos, int loss_kind,
+                            float margin_or_target, bool pin = true) {
+  // pin: the share of the entity table the TransE / TransH kernels load with evict_last (the TransR kernels take none)
+  return GroupArgs{*T, ph, pt, pr, idx_bytes == 8, corrupt, LossCfg{loss_kind, margin_or_target, n_neg, n_pos, batch_pos},
+                   pin ? l2_keep_fraction(static_cast<double>(T->n_ent) * T->ld * sizeof(float)) : 1.f};
+}
+
+// The register kernels k_group_step_e / _h take TransE / TransH rows of d <= 128 and at most 32 negatives (a group's
+// ids and saved scores are held one per lane), with slot offsets and score indices in 32 bits.  Every other shape runs
+// the general kernel k_group_step.
+static bool group_on_registers(const Plan& pl, const kgrec_tables* T, int64_t n_pos, int32_t n_neg) {
+  return (pl.fam == FAM_E || pl.fam == FAM_H) && pl.nch == 1 && n_neg <= 32 &&
+         static_cast<double>(n_pos) * (2 + n_neg) * T->dim * 4 < 4.0e9 && static_cast<double>(n_pos) * n_neg < 2.0e9;
+}
+
+enum { MODE_FWD = 0, MODE_BWD = 1, MODE_STEP = 2 };
+
+using GroupRegKernel = void (*)(GroupArgs, float, const float*, float*, float*, float*, kgrec_grads, int64_t*, int64_t*,
+                                int32_t*);
+using GroupKernel = void (*)(GroupArgs, float, float*, float*, float*, kgrec_grads, int32_t*, const float*);
+
+// k_group_step_e / _h of family FAM for the runtime flags (l1, dense, margin), bound one at a time into F, and for
+// (reg, mode).  A mode pins the flags it ignores -- FWD writes no gradient (dense = false), the fused regulariser goes
+// with the margin loss only -- so a family has 8 STEP + 4 REG + 4 FWD + 8 BWD instantiations.
+template <int FAM, bool... F>
+static GroupRegKernel group_reg_kernel(const bool (&flag)[3], bool reg, int mode) {
+  if constexpr (sizeof...(F) < 3) {
+    return flag[sizeof...(F)] ? group_reg_kernel<FAM, F..., true>(flag, reg, mode)
+                              : group_reg_kernel<FAM, F..., false>(flag, reg, mode);
+  } else {
+    constexpr bool f[] = {F...};
+    constexpr bool L1 = f[0], DENSE = f[1], MARGIN = f[2];
+    if constexpr (FAM == FAM_E) {
+      if (mode == MODE_FWD) return k_group_step_e<L1, false, MARGIN, false, false, true>;
+      if (mode == MODE_BWD) return k_group_step_e<L1, DENSE, MARGIN, false, true, false>;
+      return reg ? k_group_step_e<L1, DENSE, true, true, false, false> : k_group_step_e<L1, DENSE, MARGIN, false, false, false>;
+    } else {
+      if (mode == MODE_FWD) return k_group_step_h<L1, false, MARGIN, false, false, true>;
+      if (mode == MODE_BWD) return k_group_step_h<L1, DENSE, MARGIN, false, true, false>;
+      return reg ? k_group_step_h<L1, DENSE, true, true, false, false> : k_group_step_h<L1, DENSE, MARGIN, false, false, false>;
+    }
+  }
+}
+
+template <int FAM, int NCH>
+static GroupKernel group_kernel(bool l1, int mode) {
+  if (mode == MODE_FWD) return l1 ? k_group_step<FAM, NCH, true, false, true> : k_group_step<FAM, NCH, false, false, true>;
+  if (mode == MODE_BWD) return l1 ? k_group_step<FAM, NCH, true, true> : k_group_step<FAM, NCH, false, true>;
+  return l1 ? k_group_step<FAM, NCH, true> : k_group_step<FAM, NCH, false>;
+}
+
+// One launch of the TransE / TransH group kernels in `mode`: the register kernels where group_on_registers allows,
+// the general kernel (and k_group_slot_ids for the slot row ids) elsewhere.  FWD leaves Gr unused; BWD reads the saved
+// pos / neg scores and up0 * up_dev[batch] as the upstream, and writes neither losses nor the status word.
+static void launch_group(const Plan& pl, const GroupArgs& G, int mode, bool reg, float up0, const float* up_dev,
+                         float* pos_scores, float* neg_scores, float* group_loss, const kgrec_grads& Gr,
+                         int64_t* slot_ent, int64_t* slot_rel, int32_t* status, cudaStream_t st) {
+  const int64_t n_pos = G.L.n_pos;
+  const int n_neg = G.L.n_neg;
+  if (group_on_registers(pl, &G.T, n_pos, n_neg)) {
+    const bool flag[3] = {G.T.l1 != 0, Gr.mode == 1, G.L.kind == KGREC_LOSS_MARGIN};
+    const GroupRegKernel kern = pl.fam == FAM_E ? group_reg_kernel<FAM_E>(flag, reg, mode) : group_reg_kernel<FAM_H>(flag, reg, mode);
+    kern<<<grid_for(n_pos), kThreads, 0, st>>>(G, up0, up_dev, pos_scores, neg_scores, group_loss, Gr, slot_ent, slot_rel, status);
+    return;
+  }
+  const bool l1 = G.T.l1 != 0;
+  const GroupKernel kern =
+      pl.fam == FAM_E ? (pl.nch == 1 ? group_kernel<FAM_E, 1>(l1, mode) : pl.nch == 2 ? group_kernel<FAM_E, 2>(l1, mode) : group_kernel<FAM_E, 4>(l1, mode))
+                      : (pl.nch == 1 ? group_kernel<FAM_H, 1>(l1, mode) : pl.nch == 2 ? group_kernel<FAM_H, 2>(l1, mode) : group_kernel<FAM_H, 4>(l1, mode));
+  kern<<<grid_for(n_pos), kThreads, 0, st>>>(G, up0, pos_scores, neg_scores, group_loss, Gr, status, up_dev);
+  if (slot_ent) {
+    const int64_t total = n_pos * (2 + static_cast<int64_t>(n_neg));
+    const int64_t ctas = (total + 255) / 256, cap = static_cast<int64_t>(sm_count()) * 16;
+    k_group_slot_ids<<<static_cast<unsigned>(ctas < cap ? ctas : cap), 256, 0, st>>>(G.ph, G.pt, G.pr, G.is64, G.corrupt, n_pos, n_neg,
+                                                                                       slot_ent, slot_rel);
+  }
+}
+
 }  // namespace kgrec
 
 using namespace kgrec;
-
-#define KGREC_GROUP_DISPATCH(CALL)                                            \
-  if (pl.fam == FAM_E) {                                                      \
-    if (pl.nch == 1) { CALL(FAM_E, 1) } else if (pl.nch == 2) { CALL(FAM_E, 2) } else { CALL(FAM_E, 4) } \
-  } else {                                                                    \
-    if (pl.nch == 1) { CALL(FAM_H, 1) } else if (pl.nch == 2) { CALL(FAM_H, 2) } else { CALL(FAM_H, 4) } \
-  }
 
 extern "C" int kgrec_corrupt_loss_fwd(const kgrec_tables* tables, int model, const void* ph, const void* pt,
                                       const void* pr, int idx_bytes, int64_t n_pos, const int32_t* corrupt,
@@ -1880,34 +1812,13 @@ extern "C" int kgrec_corrupt_loss_fwd(const kgrec_tables* tables, int model, con
   if (rc) return rc;
   if (!pos_scores || !neg_scores || !loss || !workspace) { set_error("output / workspace pointer is NULL"); return KGREC_ERR_INVALID; }
   if (n_pos == 0) return KGREC_OK;
-  const GroupArgs G{*tables, ph, pt, pr, idx_bytes == 8, corrupt, LossCfg{loss_kind, margin_or_target, n_neg, n_pos, batch_pos},
-                    l2_keep_fraction(static_cast<double>(tables->n_ent) * tables->ld * sizeof(float))};
+  const GroupArgs G = group_args(tables, ph, pt, pr, idx_bytes, n_pos, corrupt, n_neg, batch_pos, loss_kind, margin_or_target);
   float* group_loss = static_cast<float*>(workspace);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  const char* env = group_step_env();
-  const bool small32 = n_neg <= 32 && static_cast<double>(n_pos) * (2 + n_neg) * tables->dim * 4 < 4.0e9 &&
-                       static_cast<double>(n_pos) * n_neg < 2.0e9;
-  if ((pl.fam == FAM_E || pl.fam == FAM_H) && pl.nch == 1 && small32 && !(env && env[0] == '0')) {
-    // the step kernels in forward-only mode; for TransH this beats k_group_fwd on an H100 (d = 100, 256 batches of
-    // 1024 positives x 10 negatives: forward 0.49-0.50 vs 0.51-0.52 ms, forward + backward 1.56-1.58 vs 1.59 ms)
-    const kgrec_grads nog{};
-#define CALL_F(KERN, MINBV, L1V, MV) KERN<L1V, false, MV, MINBV, true, false, false, true><<<grid_for(n_pos), kThreads, 0, st>>>(G, 1.f, nullptr, pos_scores, neg_scores, group_loss, nog, nullptr, nullptr, status)
-#define CALL_F4(KERN, MINBV)                                                                                        \
-  {                                                                                                                 \
-    const bool mg = loss_kind == KGREC_LOSS_MARGIN;                                                                 \
-    if (tables->l1) { if (mg) CALL_F(KERN, MINBV, true, true); else CALL_F(KERN, MINBV, true, false); }             \
-    else { if (mg) CALL_F(KERN, MINBV, false, true); else CALL_F(KERN, MINBV, false, false); }                      \
-  }
-    if (pl.fam == FAM_E) CALL_F4(k_group_step_e, 4) else CALL_F4(k_group_step_h, 3)
-#undef CALL_F4
-#undef CALL_F
-  } else {
-#define CALL(FAMV, NCHV)                                                                                                  \
-  if (tables->l1) k_group_fwd<FAMV, NCHV, true><<<grid_for(n_pos), kThreads, 0, st>>>(G, pos_scores, neg_scores, group_loss, status); \
-  else k_group_fwd<FAMV, NCHV, false><<<grid_for(n_pos), kThreads, 0, st>>>(G, pos_scores, neg_scores, group_loss, status);
-  KGREC_GROUP_DISPATCH(CALL)
-#undef CALL
-  }
+  // the register kernels in forward-only mode: for TransH this beats the general kernel on an H100 (d = 100, 256 batches
+  // of 1024 positives x 10 negatives: forward 0.49-0.50 vs 0.51-0.52 ms, forward + backward 1.56-1.58 vs 1.59 ms)
+  launch_group(pl, G, MODE_FWD, false, 1.f, nullptr, pos_scores, neg_scores, group_loss, kgrec_grads{}, nullptr, nullptr,
+               status, st);
   KGREC_CUDA_OK(cudaGetLastError());
   const int64_t n_batches = (n_pos + batch_pos - 1) / batch_pos;
   k_batch_loss<<<static_cast<unsigned>(n_batches), 256, 0, st>>>(group_loss, G.L, loss);
@@ -1931,41 +1842,9 @@ extern "C" int kgrec_corrupt_loss_bwd(const kgrec_tables* tables, int model, con
     return KGREC_ERR_INVALID;
   }
   if (n_pos == 0) return KGREC_OK;
-  const GroupArgs G{*tables, ph, pt, pr, idx_bytes == 8, corrupt, LossCfg{loss_kind, margin_or_target, n_neg, n_pos, batch_pos},
-                    l2_keep_fraction(static_cast<double>(tables->n_ent) * tables->ld * sizeof(float))};
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  const char* env = group_step_env();
-  const bool small32 = n_neg <= 32 && static_cast<double>(n_pos) * (2 + n_neg) * tables->dim * 4 < 4.0e9 &&
-                       static_cast<double>(n_pos) * n_neg < 2.0e9;
-  if ((pl.fam == FAM_E || pl.fam == FAM_H) && pl.nch == 1 && small32 && !(env && env[0] == '0')) {
-    // the step kernels in backward mode (coefficients from the saved scores, upstream per batch)
-    float* ps = const_cast<float*>(pos_scores);
-    float* ns = const_cast<float*>(neg_scores);
-#define CALL_B(KERN, MINBV, L1V, DV, MV) KERN<L1V, DV, MV, MINBV, true, false, true><<<grid_for(n_pos), kThreads, 0, st>>>(G, grad_loss, grad_loss_dev, ps, ns, nullptr, *grads, slot_ent_ids, slot_rel_ids, nullptr)
-#define CALL_B8(KERN, MINBV)                                                                                                   \
-  {                                                                                                                            \
-    const bool dn = grads->mode == 1, mg = loss_kind == KGREC_LOSS_MARGIN;                                                     \
-    if (tables->l1) { if (dn) { if (mg) CALL_B(KERN, MINBV, true, true, true); else CALL_B(KERN, MINBV, true, true, false); }  \
-                      else { if (mg) CALL_B(KERN, MINBV, true, false, true); else CALL_B(KERN, MINBV, true, false, false); } } \
-    else { if (dn) { if (mg) CALL_B(KERN, MINBV, false, true, true); else CALL_B(KERN, MINBV, false, true, false); }           \
-           else { if (mg) CALL_B(KERN, MINBV, false, false, true); else CALL_B(KERN, MINBV, false, false, false); } }          \
-  }
-    if (pl.fam == FAM_E) CALL_B8(k_group_step_e, 4) else CALL_B8(k_group_step_h, 3)
-#undef CALL_B8
-#undef CALL_B
-  } else {
-#define CALL(FAMV, NCHV)                                                                                                  \
-  if (tables->l1) k_group_bwd<FAMV, NCHV, true><<<grid_for(n_pos), kThreads, 0, st>>>(G, pos_scores, neg_scores, grad_loss, grad_loss_dev, *grads); \
-  else k_group_bwd<FAMV, NCHV, false><<<grid_for(n_pos), kThreads, 0, st>>>(G, pos_scores, neg_scores, grad_loss, grad_loss_dev, *grads);
-  KGREC_GROUP_DISPATCH(CALL)
-#undef CALL
-    if (slot_ent_ids) {
-      const int64_t total = n_pos * (2 + static_cast<int64_t>(n_neg));
-      const int64_t ctas = (total + 255) / 256, cap = static_cast<int64_t>(sm_count()) * 16;
-      k_group_slot_ids<<<static_cast<unsigned>(ctas < cap ? ctas : cap), 256, 0, st>>>(ph, pt, pr, idx_bytes == 8, corrupt, n_pos, n_neg,
-                                                                                         slot_ent_ids, slot_rel_ids);
-    }
-  }
+  const GroupArgs G = group_args(tables, ph, pt, pr, idx_bytes, n_pos, corrupt, n_neg, batch_pos, loss_kind, margin_or_target);
+  launch_group(pl, G, MODE_BWD, false, grad_loss, grad_loss_dev, const_cast<float*>(pos_scores), const_cast<float*>(neg_scores),
+               nullptr, *grads, slot_ent_ids, slot_rel_ids, nullptr, static_cast<cudaStream_t>(stream));
   KGREC_CUDA_OK(cudaGetLastError());
   return KGREC_OK;
 }
@@ -1994,32 +1873,39 @@ extern "C" int kgrec_corrupt_loss_step(const kgrec_tables* tables, int model, co
   if ((slot_ent_ids == nullptr) != (slot_rel_ids == nullptr)) { set_error("slot_ent_ids and slot_rel_ids go together"); return KGREC_ERR_INVALID; }
   if (reg_flags != 0 && reg_flags != 1) { set_error("reg_flags must be 0 or 1"); return KGREC_ERR_INVALID; }
   if (reg_flags && loss_kind != KGREC_LOSS_MARGIN) { set_error("fused regularisers go with the margin loss (the KG drivers' loss)"); return KGREC_ERR_UNSUPPORTED; }
+  if (pl.fam == FAM_R && (pl.nch != 1 || n_neg > 14)) {
+    set_error("TransR step kernel: embedding_size <= 128 and at most 14 negatives per positive");
+    return KGREC_ERR_UNSUPPORTED;
+  }
+  if (n_pos == 0) return KGREC_OK;
+  const bool on_registers = group_on_registers(pl, tables, n_pos, n_neg);
+  if (reg_flags && pl.fam != FAM_R && !on_registers) {
+    set_error("fused regularisers are built for the d <= 128 margin-loss step kernels only");
+    return KGREC_ERR_UNSUPPORTED;
+  }
+  const GroupArgs G = group_args(tables, ph, pt, pr, idx_bytes, n_pos, corrupt, n_neg, batch_pos, loss_kind, margin_or_target,
+                                 pl.fam != FAM_R);
+  float* group_loss = static_cast<float*>(workspace);
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const bool mg = loss_kind == KGREC_LOSS_MARGIN;
+  // slot gradients of TransE at d <= 128 without the fused regulariser: the TMA-staged gather when its ring fits and
+  // every warp gets at least two groups (with one, the second stage has nothing to overlap and a single 1024-positive
+  // batch runs faster on the register kernel)
+  const bool tma = pl.fam == FAM_E && on_registers && grads->mode == 0 && !reg_flags && n_neg <= 29 &&
+                   tables->ld == tables->dim && group_step_tma_smem(tables->dim, n_neg) <= 225 * 1024 &&
+                   n_pos >= static_cast<int64_t>(kTmaStages) * kTmaWarps * sm_count();
   if (pl.fam == FAM_R) {
-    if (pl.nch != 1 || n_neg > 14) { set_error("TransR step kernel: embedding_size <= 128 and at most 14 negatives per positive"); return KGREC_ERR_UNSUPPORTED; }
-    if (n_pos == 0) return KGREC_OK;
-    const GroupArgs GA{*tables, ph, pt, pr, idx_bytes == 8, corrupt, LossCfg{loss_kind, margin_or_target, n_neg, n_pos, batch_pos}, 1.f};
-    float* gl = static_cast<float*>(workspace);
-    cudaStream_t s2 = static_cast<cudaStream_t>(stream);
-    // workspace: [group_loss n_pos | order n_pos | cursor n_rel]
-    int32_t* order = reinterpret_cast<int32_t*>(gl + n_pos);
+    // workspace: [group_loss n_pos | order n_pos | cursor n_rel]; the groups in relation order
+    int32_t* order = reinterpret_cast<int32_t*>(group_loss + n_pos);
     int32_t* cursor = order + n_pos;
-    {
-      const char* env = group_step_env();
-      if (env && env[0] == 'u') order = nullptr;                      // KGREC_GROUP_STEP=u: batch order (A/B)
-    }
-    if (order) {
-      KGREC_CUDA_OK(cudaMemsetAsync(cursor, 0, sizeof(int32_t) * tables->n_rel, s2));
-      const int gs = static_cast<int>((n_pos + 255) / 256 < sm_count() * 4 ? (n_pos + 255) / 256 : sm_count() * 4);
-      k_rel_hist<<<gs, 256, 0, s2>>>(pr, idx_bytes == 8, static_cast<int>(n_pos), tables->n_rel, cursor);
-      k_rel_scan<<<1, 1024, 0, s2>>>(cursor, tables->n_rel);
-      k_rel_scatter<<<gs, 256, 0, s2>>>(pr, idx_bytes == 8, static_cast<int>(n_pos), tables->n_rel, cursor, order);
-    }
-    const bool mg = loss_kind == KGREC_LOSS_MARGIN;
-    const char* env_r = group_step_env();
+    KGREC_CUDA_OK(cudaMemsetAsync(cursor, 0, sizeof(int32_t) * tables->n_rel, st));
+    const int gs = static_cast<int>((n_pos + 255) / 256 < sm_count() * 4 ? (n_pos + 255) / 256 : sm_count() * 4);
+    k_rel_hist<<<gs, 256, 0, st>>>(pr, idx_bytes == 8, static_cast<int>(n_pos), tables->n_rel, cursor);
+    k_rel_scan<<<1, 1024, 0, st>>>(cursor, tables->n_rel);
+    k_rel_scatter<<<gs, 256, 0, st>>>(pr, idx_bytes == 8, static_cast<int>(n_pos), tables->n_rel, cursor, order);
     // short runs (fewer than ~4 groups per relation of the table): staging M_r per tile does not pay, the warp kernel stays
-    const bool long_runs = n_pos >= 4 * tables->n_rel || (env_r && env_r[0] == 'r');
-    if (tables->dim >= 32 && long_runs && !(env_r && (env_r[0] == 'w' || env_r[0] == 'u'))) {
-      // the CTA-level run kernel; KGREC_GROUP_STEP=w keeps the warp-per-group kernel (A/B), =u that kernel in batch order
+    if (tables->dim >= 32 && n_pos >= 4 * tables->n_rel) {
+      // the CTA-level run kernel
       const int d = tables->dim, NC = d / 4, pitch = run_pitch(d), qf = d / 32;
       auto smem_for = [&](int rb) { return (2 * static_cast<size_t>(d) + 2 * 64 * rb) * pitch * 4 + 3 * 64 * rb * 8 + 72 * 4; };
       const int rb = (NC <= 27 && smem_for(2) <= 220 * 1024) ? 2 : 1;
@@ -2031,52 +1917,29 @@ extern "C" int kgrec_corrupt_loss_step(const kgrec_tables* tables, int model, co
     auto kern = reg_flags ? k_run_step_r<QAV, QBV, QFV, RBV, true, true>                                                 \
                           : (mg ? k_run_step_r<QAV, QBV, QFV, RBV, true, false> : k_run_step_r<QAV, QBV, QFV, RBV, false, false>); \
     KGREC_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));       \
-    kern<<<grid, kThreads, smem, s2>>>(GA, grad_loss, pos_scores, neg_scores, gl, *grads, slot_ent_ids, slot_rel_ids, status, order); \
+    kern<<<grid, kThreads, smem, st>>>(G, grad_loss, pos_scores, neg_scores, group_loss, *grads, slot_ent_ids, slot_rel_ids, status, order); \
   }
       if (NC <= 16) { if (qf <= 1) CALL_RUN(1, 1, 1, 2) else CALL_RUN(1, 1, 2, 2) }
       else if (NC <= 27) { if (qf <= 2) CALL_RUN(1, 3, 2, 2) else CALL_RUN(1, 3, 3, 2) }
       else { if (qf <= 3) CALL_RUN(2, 2, 3, 1) else CALL_RUN(2, 2, 4, 1) }
 #undef CALL_RUN
     } else {
-    const int64_t want = (n_pos + kWarpsPerCta - 1) / kWarpsPerCta;
-    const int grid_r = static_cast<int>(want < sm_count() ? want : sm_count());          // one resident CTA per SM
-    const int nvt = n_neg <= 2 ? 4 : (n_neg <= 10 ? 12 : 16);
-    const size_t smem = static_cast<size_t>(kWarpsPerCta) * (static_cast<size_t>(nvt) * (tables->dim / 4) + static_cast<size_t>(tables->dim) * (nvt / 4)) * 16;
+      const int64_t want = (n_pos + kWarpsPerCta - 1) / kWarpsPerCta;
+      const int grid_r = static_cast<int>(want < sm_count() ? want : sm_count());          // one resident CTA per SM
+      const int nvt = n_neg <= 2 ? 4 : (n_neg <= 10 ? 12 : 16);
+      const size_t smem = static_cast<size_t>(kWarpsPerCta) * (static_cast<size_t>(nvt) * (tables->dim / 4) + static_cast<size_t>(tables->dim) * (nvt / 4)) * 16;
 #define CALL_R(NVTV, MV, RV)                                                                                         \
   {                                                                                                                  \
     auto kern = k_group_step_r<NVTV, MV, RV>;                                                                        \
     KGREC_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));   \
-    kern<<<grid_r, kThreads, smem, s2>>>(GA, grad_loss, pos_scores, neg_scores, gl, *grads, slot_ent_ids, slot_rel_ids, status, order); \
+    kern<<<grid_r, kThreads, smem, st>>>(G, grad_loss, pos_scores, neg_scores, group_loss, *grads, slot_ent_ids, slot_rel_ids, status, order); \
   }
-    if (nvt == 4) { if (reg_flags) CALL_R(4, true, true) else if (mg) CALL_R(4, true, false) else CALL_R(4, false, false) }
-    else if (nvt == 12) { if (reg_flags) CALL_R(12, true, true) else if (mg) CALL_R(12, true, false) else CALL_R(12, false, false) }
-    else { if (reg_flags) CALL_R(16, true, true) else if (mg) CALL_R(16, true, false) else CALL_R(16, false, false) }
+      if (nvt == 4) { if (reg_flags) CALL_R(4, true, true) else if (mg) CALL_R(4, true, false) else CALL_R(4, false, false) }
+      else if (nvt == 12) { if (reg_flags) CALL_R(12, true, true) else if (mg) CALL_R(12, true, false) else CALL_R(12, false, false) }
+      else { if (reg_flags) CALL_R(16, true, true) else if (mg) CALL_R(16, true, false) else CALL_R(16, false, false) }
 #undef CALL_R
     }
-    KGREC_CUDA_OK(cudaGetLastError());
-    const int64_t nbt = (n_pos + batch_pos - 1) / batch_pos;
-    k_batch_loss<<<static_cast<unsigned>(nbt), 256, 0, s2>>>(gl, GA.L, loss);
-    KGREC_CUDA_OK(cudaGetLastError());
-    return KGREC_OK;
-  }
-  if (n_pos == 0) return KGREC_OK;
-  const GroupArgs G{*tables, ph, pt, pr, idx_bytes == 8, corrupt, LossCfg{loss_kind, margin_or_target, n_neg, n_pos, batch_pos},
-                    l2_keep_fraction(static_cast<double>(tables->n_ent) * tables->ld * sizeof(float))};
-  float* group_loss = static_cast<float*>(workspace);
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  // KGREC_GROUP_STEP (A/B runs, tests): 0 = the general kernel for every shape; n = no row prefetch;
-  // 3 (TransE) / 2 (TransH) = fewer CTAs per SM, no prefetch
-  const char* env = group_step_env();
-  const bool small32 = n_neg <= 32 && static_cast<double>(n_pos) * (2 + n_neg) * tables->dim * 4 < 4.0e9 &&
-                       static_cast<double>(n_pos) * n_neg < 2.0e9;          // 32-bit slot offsets, scores kept in lanes
-  // slot gradients of TransE at d <= 128 without the fused regulariser: the TMA-staged gather when its ring fits and
-  // every warp gets at least two groups (with one, the second stage has nothing to overlap and a single 1024-positive
-  // batch runs faster on the register kernel); KGREC_GROUP_STEP = 0 / n / 3 keep the general or register kernels
-  const bool tma = pl.fam == FAM_E && pl.nch == 1 && small32 && grads->mode == 0 && !reg_flags && n_neg <= 29 &&
-                   tables->ld == tables->dim && !(env && (env[0] == '0' || env[0] == 'n' || env[0] == '3')) &&
-                   group_step_tma_smem(tables->dim, n_neg) <= 225 * 1024 &&
-                   n_pos >= static_cast<int64_t>(kTmaStages) * kTmaWarps * sm_count();
-  if (tma) {
+  } else if (tma) {
     const size_t smem = group_step_tma_smem(tables->dim, n_neg);
     int64_t ctas = (n_pos + kTmaWarps - 1) / kTmaWarps;
     if (ctas > sm_count()) ctas = sm_count();
@@ -2087,56 +1950,13 @@ extern "C" int kgrec_corrupt_loss_step(const kgrec_tables* tables, int model, co
     kern<<<static_cast<int>(ctas), kTmaWarps * 32, smem, st>>>(G, grad_loss, pos_scores, neg_scores, group_loss, *grads, slot_ent_ids, slot_rel_ids, status, kTmaStages); \
   }
 #define CALL_TN(L1V, MV) { if (n_neg < 16) CALL_T(L1V, MV, 16) else CALL_T(L1V, MV, 32) }
-    const bool mg = loss_kind == KGREC_LOSS_MARGIN;
     if (tables->l1) { if (mg) CALL_TN(true, true) else CALL_TN(true, false) }
     else { if (mg) CALL_TN(false, true) else CALL_TN(false, false) }
 #undef CALL_TN
 #undef CALL_T
-  } else if (pl.fam == FAM_E && pl.nch == 1 && small32 && !(env && env[0] == '0')) {
-#define CALL_E(L1V, DV, MV)                                                                                      \
-  {                                                                                                              \
-    if (env && env[0] == 'n')                                                                                    \
-      k_group_step_e<L1V, DV, MV, 4, false, false, false><<<grid_for(n_pos), kThreads, 0, st>>>(G, grad_loss, nullptr, pos_scores, neg_scores, group_loss, *grads, slot_ent_ids, slot_rel_ids, status); \
-    else if (env && env[0] == '3')                                                                               \
-      k_group_step_e<L1V, DV, MV, 3, false, false, false><<<grid_for(n_pos), kThreads, 0, st>>>(G, grad_loss, nullptr, pos_scores, neg_scores, group_loss, *grads, slot_ent_ids, slot_rel_ids, status); \
-    else if (MV && reg_flags)                                                                                    \
-      k_group_step_e<L1V, DV, true, 4, true, true, false><<<grid_for(n_pos), kThreads, 0, st>>>(G, grad_loss, nullptr, pos_scores, neg_scores, group_loss, *grads, slot_ent_ids, slot_rel_ids, status); \
-    else                                                                                                         \
-      k_group_step_e<L1V, DV, MV, 4, true, false, false><<<grid_for(n_pos), kThreads, 0, st>>>(G, grad_loss, nullptr, pos_scores, neg_scores, group_loss, *grads, slot_ent_ids, slot_rel_ids, status); \
-  }
-    const bool dn = grads->mode == 1, mg = loss_kind == KGREC_LOSS_MARGIN;
-    if (tables->l1) { if (dn) { if (mg) CALL_E(true, true, true) else CALL_E(true, true, false) } else { if (mg) CALL_E(true, false, true) else CALL_E(true, false, false) } }
-    else { if (dn) { if (mg) CALL_E(false, true, true) else CALL_E(false, true, false) } else { if (mg) CALL_E(false, false, true) else CALL_E(false, false, false) } }
-#undef CALL_E
-  } else if (pl.fam == FAM_H && pl.nch == 1 && small32 && !(env && env[0] == '0')) {
-#define CALL_H(L1V, DV, MV)                                                                                      \
-  {                                                                                                              \
-    if (env && env[0] == 'n')                                                                                    \
-      k_group_step_h<L1V, DV, MV, 3, false, false, false><<<grid_for(n_pos), kThreads, 0, st>>>(G, grad_loss, nullptr, pos_scores, neg_scores, group_loss, *grads, slot_ent_ids, slot_rel_ids, status); \
-    else if (env && env[0] == '2')                                                                               \
-      k_group_step_h<L1V, DV, MV, 2, false, false, false><<<grid_for(n_pos), kThreads, 0, st>>>(G, grad_loss, nullptr, pos_scores, neg_scores, group_loss, *grads, slot_ent_ids, slot_rel_ids, status); \
-    else if (MV && reg_flags)                                                                                    \
-      k_group_step_h<L1V, DV, true, 3, true, true, false><<<grid_for(n_pos), kThreads, 0, st>>>(G, grad_loss, nullptr, pos_scores, neg_scores, group_loss, *grads, slot_ent_ids, slot_rel_ids, status); \
-    else                                                                                                         \
-      k_group_step_h<L1V, DV, MV, 3, true, false, false><<<grid_for(n_pos), kThreads, 0, st>>>(G, grad_loss, nullptr, pos_scores, neg_scores, group_loss, *grads, slot_ent_ids, slot_rel_ids, status); \
-  }
-    const bool dn = grads->mode == 1, mg = loss_kind == KGREC_LOSS_MARGIN;
-    if (tables->l1) { if (dn) { if (mg) CALL_H(true, true, true) else CALL_H(true, true, false) } else { if (mg) CALL_H(true, false, true) else CALL_H(true, false, false) } }
-    else { if (dn) { if (mg) CALL_H(false, true, true) else CALL_H(false, true, false) } else { if (mg) CALL_H(false, false, true) else CALL_H(false, false, false) } }
-#undef CALL_H
   } else {
-    if (reg_flags) { set_error("fused regularisers are built for the d <= 128 margin-loss step kernels only"); return KGREC_ERR_UNSUPPORTED; }
-#define CALL(FAMV, NCHV)                                                                                        \
-  if (tables->l1) k_group_step<FAMV, NCHV, true><<<grid_for(n_pos), kThreads, 0, st>>>(G, grad_loss, pos_scores, neg_scores, group_loss, *grads, status); \
-  else k_group_step<FAMV, NCHV, false><<<grid_for(n_pos), kThreads, 0, st>>>(G, grad_loss, pos_scores, neg_scores, group_loss, *grads, status);
-  KGREC_GROUP_DISPATCH(CALL)
-#undef CALL
-    if (slot_ent_ids) {
-      const int64_t total = n_pos * (2 + static_cast<int64_t>(n_neg));
-      const int64_t ctas = (total + 255) / 256, cap = static_cast<int64_t>(sm_count()) * 16;
-      k_group_slot_ids<<<static_cast<unsigned>(ctas < cap ? ctas : cap), 256, 0, st>>>(ph, pt, pr, idx_bytes == 8, corrupt, n_pos, n_neg,
-                                                                                         slot_ent_ids, slot_rel_ids);
-    }
+    launch_group(pl, G, MODE_STEP, reg_flags != 0, grad_loss, nullptr, pos_scores, neg_scores, group_loss, *grads,
+                 slot_ent_ids, slot_rel_ids, status, st);
   }
   KGREC_CUDA_OK(cudaGetLastError());
   const int64_t n_batches = (n_pos + batch_pos - 1) / batch_pos;

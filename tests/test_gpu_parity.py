@@ -534,15 +534,17 @@ def test_step_with_fused_regularisers(cls_name, l1):
 
 
 @pytest.mark.parametrize("cls_name", ["TransEModel", "TransHModel"])
-@pytest.mark.parametrize("Kn", [1, 2, 31, 32, 40])
-def test_step_kernel_negative_counts(cls_name, Kn):
+@pytest.mark.parametrize("Kn,d", [pytest.param(kn, 64, id=str(kn)) for kn in (1, 2, 31, 32, 40)] +
+                         [pytest.param(kn, d, id="%d-d%d" % (kn, d)) for kn, d in ((2, 200), (40, 200), (1, 512), (40, 512))])
+def test_step_kernel_negative_counts(cls_name, Kn, d):
     """The step kernels hold a group's corrupted ids one per lane: 1 and 2 negatives (the reference's own 1 per
     positive), the lane-count edges 31 / 32, and 40 (falls back to the general kernel) against the two-kernel
-    autograd path on the same inputs; the slot row ids are checked through the sparse gradients."""
+    autograd path on the same inputs; the slot row ids are checked through the sparse gradients.  d = 200 and 512
+    run the general kernel's step, forward and backward modes with two and four 128-wide chunks per row."""
     import kgrec_b200 as K
     torch.manual_seed(Kn)
     rng = np.random.RandomState(Kn)
-    d, E, R, n_pos, bp = 64, 700, 5, 517, 128
+    E, R, n_pos, bp = 700, 5, 517, 128
     m = getattr(K, cls_name)(Kn % 2 == 0, d, E, R)
     h, t, r = rng.randint(0, E, n_pos), rng.randint(0, E, n_pos), rng.randint(0, R, n_pos)
     ce = rng.randint(0, E, n_pos * Kn)
@@ -834,7 +836,7 @@ def test_eval_scores_independent_of_row_position(d):
 @pytest.mark.parametrize("cls_name", ["TransEModel", "TransHModel"])
 @pytest.mark.parametrize("l1", [False, True])
 @pytest.mark.parametrize("loss,param", [("margin", 1.0), ("bpr", -1.0)])
-@pytest.mark.parametrize("d", [100, 200])
+@pytest.mark.parametrize("d", [100, 200, 512])
 def test_corrupt_format_matches_expanded_triples(cls_name, l1, loss, param, d):
     """The group-compact negative format gives the same scores, losses and gradients as the
     expanded (nh, nt, nr) triples, and both match the oracle."""

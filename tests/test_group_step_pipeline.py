@@ -3,7 +3,8 @@ read before its stage is refilled, one reduce-scatter for the 1 + K scores, coef
 
 Every case runs on the TMA side of the dispatch (sparse slot gradients, no fused regulariser, ring within 225 KB, at least
 two groups per warp) and is compared bit for bit -- losses, positive and negative scores, every slot value and the COO
-ids -- with the register kernel k_group_step_e (KGREC_GROUP_STEP=n) run in a child process.  The cases cover:
+ids -- with the register kernel k_group_step_e, run on the same inputs cut at batch boundaries into launches too small
+for the TMA kernel.  The cases cover:
   * 1 + K <= 16 (the 16-slot reduce-scatter, rows kept in registers), 1 + K = 17 (the 32-slot reduce-scatter crosses
     a half-warp) and K = 29 (the largest K this kernel takes; rows read twice);
   * d in {4, 36, 100, 128}, L1 and L2, margin and BPR, int32 and int64 ids;
@@ -11,7 +12,6 @@ ids -- with the register kernel k_group_step_e (KGREC_GROUP_STEP=n) run in a chi
 One more test puts an out-of-range id in a batch: the kernel clamps it, raises the status word and does not fault.
 """
 import os
-import subprocess
 import sys
 
 import numpy as np
@@ -86,7 +86,13 @@ def make_inputs(c, seed):
     return h, t, r, cid, torch.where(head, ~cid, cid)
 
 
-def run_case(c):
+def slices(n_pos):
+    """[lo, hi) ranges of whole loss batches, each of fewer positives than the smallest TMA launch."""
+    step = (smallest_launch() - 1) // BATCH_POS * BATCH_POS
+    return [(lo, min(n_pos, lo + step)) for lo in range(0, n_pos, step)]
+
+
+def run_case(c, rows=None):      # rows = (j0, j1): only positives j0 .. j1 - 1 (whole batches) and their negatives
     import kgrec_b200 as K
     d, k, l1, loss, _, _ = c
     seed = 2000 + CASES.index(c)
@@ -94,9 +100,11 @@ def run_case(c):
     m = K.TransEModel(l1, d, N_ENT, N_REL)
     m.grad_mode = "sparse"
     h, t, r, cid, corrupt = make_inputs(c, seed)
+    j0, j1 = rows if rows is not None else (0, h.numel())
     param = 1.0 if loss == "margin" else 0.5
     kw = {"margin": param} if loss == "margin" else {"loss": "bpr", "margin": param}
-    lo, ps, ns = m.loss_step_corrupt(tuple(x.cuda() for x in (h, t, r)), corrupt.cuda(), batch_pos=BATCH_POS, **kw)
+    lo, ps, ns = m.loss_step_corrupt(tuple(x[j0:j1].cuda() for x in (h, t, r)), corrupt[j0 * k:j1 * k].cuda(),
+                                     batch_pos=BATCH_POS, **kw)
     m.check_indices()
     torch.cuda.synchronize()
     out = {"loss": lo, "pos": ps, "neg": ns}
@@ -107,25 +115,26 @@ def run_case(c):
     return {key: v.cpu().numpy() for key, v in out.items()}, (h, t, r, cid)
 
 
-def dump_register_values(path):
-    """Child process (KGREC_GROUP_STEP=n): every output of the register kernel for every case."""
-    assert os.environ.get("KGREC_GROUP_STEP") == "n"
+@pytest.fixture(scope="module")
+def register_values():
+    """Every output of k_group_step_e for every case: a group's slot values and scores do not depend on the launch, and
+    slices of whole batches keep each batch's loss (BPR's per-batch count included), so the slices concatenated are
+    the outputs of the whole case."""
+    from torch.profiler import ProfilerActivity, profile
+    for _ in range(3):          # a capture whose kernel records the profiler lost names no kernel of ours: take it again
+        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            run_case(CASES[0], slices(n_pos_of(CASES[0]))[0])
+            torch.cuda.synchronize()
+        names = " ".join(e.key for e in prof.key_averages())
+        if "kgrec::" in names:
+            break
+    assert "k_group_step_e" in names and "k_group_step_e_tma" not in names, names
     out = {}
     for c in CASES:
-        vals, _ = run_case(c)
-        out.update({case_id(c) + "/" + key: v for key, v in vals.items()})
-    np.savez(path, **out)
-
-
-@pytest.fixture(scope="module")
-def register_values(tmp_path_factory):
-    path = str(tmp_path_factory.mktemp("regkernel") / "values.npz")
-    env = dict(os.environ, KGREC_GROUP_STEP="n")
-    r = subprocess.run([sys.executable, os.path.abspath(__file__), "--dump", path], env=env, cwd=ROOT,
-                       capture_output=True, text=True, timeout=900)
-    assert r.returncode == 0, r.stdout + r.stderr
-    with np.load(path) as z:
-        return {key: z[key] for key in z.files}
+        parts = [run_case(c, rows)[0] for rows in slices(n_pos_of(c))]
+        out[case_id(c)] = {key: np.concatenate([p[key] for p in parts], axis=1 if key.endswith("_ids") else 0)
+                           for key in parts[0]}
+    return out
 
 
 @pytest.mark.parametrize("c", CASES, ids=case_id)
@@ -133,7 +142,7 @@ def test_pipeline_matches_register_kernel(c, register_values):
     k = c[1]
     got, (h, t, r, cid) = run_case(c)
     for key, v in got.items():
-        want = register_values[case_id(c) + "/" + key]
+        want = register_values[case_id(c)][key]
         assert v.shape == want.shape and v.dtype == want.dtype, key
         assert np.array_equal(v.view(np.uint8), want.view(np.uint8)), key
     want_ent = torch.cat([h.long().view(-1, 1), t.long().view(-1, 1), cid.long().view(-1, k)], dim=1).view(1, -1)
@@ -184,10 +193,3 @@ def test_pipeline_out_of_range_id_raises_status(where):
         m.check_indices()
     m.check_indices()            # the word was cleared by the raise
     assert bool(torch.isfinite(lo).all()) and bool(torch.isfinite(ps).all()) and bool(torch.isfinite(ns).all())
-
-
-if __name__ == "__main__":
-    if len(sys.argv) == 3 and sys.argv[1] == "--dump":
-        dump_register_values(sys.argv[2])
-    else:
-        sys.exit("usage: test_group_step_pipeline.py --dump OUT.npz")

@@ -6,11 +6,10 @@ batches of 100 (not aligned to the 16 groups a CTA takes at a time) and checks, 
   * losses, positive and negative scores are bit for bit those of the dense-mode call (k_group_step_e, same process);
   * the densified gradients match the dense-mode gradients (atomics there: equal up to the order of the sums);
   * the COO row ids are [h, t, corrupted_1..K] per group and r per group;
-  * without the fused regulariser, the slot values are bit for bit those of the register kernel
-    (KGREC_GROUP_STEP=n, which has no regulariser variant) run in a child process.
+  * without the fused regulariser, the slot values are bit for bit those of the register kernel k_group_step_e, run on
+    the same inputs cut at batch boundaries into launches too small for the TMA kernel.
 """
 import os
-import subprocess
 import sys
 
 import numpy as np
@@ -57,7 +56,14 @@ def case_id(c):
     return "d%d-k%d-%s-%s%s-%s" % (d, k, "l1" if l1 else "l2", loss, "-withreg" if reg else "", kernel_side(d, k, reg))
 
 
-def run_case(c, mode):
+def slices(n_pos):
+    """[lo, hi) ranges of whole loss batches, each of fewer positives than the smallest TMA launch (2 x 16 x SMs)."""
+    step = (2 * 16 * torch.cuda.get_device_properties(0).multi_processor_count - 1) // BATCH_POS * BATCH_POS
+    return [(lo, min(n_pos, lo + step)) for lo in range(0, n_pos, step)]
+
+
+def run_case(c, mode, rows=None):
+    """Case c in grad mode `mode`; `rows` = (lo, hi): only positives lo .. hi - 1 (whole batches) and their negatives."""
     import kgrec_b200 as K
     d, k, l1, loss, reg = c
     seed = 1000 + CASES.index(c)
@@ -72,6 +78,9 @@ def run_case(c, mode):
     head = torch.rand(N_POS * k, generator=g) < 0.5
     corrupt = torch.where(head, ~cid, cid)
     dev = [x.cuda() for x in (h, t, r, corrupt)]
+    if rows is not None:
+        j0, j1 = rows
+        dev = [x[j0:j1] for x in dev[:3]] + [dev[3][j0 * k:j1 * k]]
     param = 1.0 if loss == "margin" else 0.5
     kw = {"margin": param} if loss == "margin" else {"loss": "bpr", "margin": param}
     lo, ps, ns = m.loss_step_corrupt(tuple(dev[:3]), dev[3], batch_pos=BATCH_POS, reg=reg, **kw)
@@ -80,28 +89,26 @@ def run_case(c, mode):
     return m, (lo, ps, ns), (h, t, r, cid)
 
 
-def dump_register_values(path):
-    """Child process (KGREC_GROUP_STEP=n): slot values of the register kernel for every case without REG."""
-    assert os.environ.get("KGREC_GROUP_STEP") == "n"
-    out = {}
-    for c in CASES:
-        if c[4]:
-            continue
-        m, _, _ = run_case(c, "sparse")
-        out[case_id(c) + "/ent"] = m.ent_embeddings.weight.grad._values().cpu().numpy()
-        out[case_id(c) + "/rel"] = m.rel_embeddings.weight.grad._values().cpu().numpy()
-    np.savez(path, **out)
-
-
 @pytest.fixture(scope="module")
-def register_values(tmp_path_factory):
-    path = str(tmp_path_factory.mktemp("regkernel") / "values.npz")
-    env = dict(os.environ, KGREC_GROUP_STEP="n")
-    r = subprocess.run([sys.executable, os.path.abspath(__file__), "--dump", path], env=env, cwd=ROOT,
-                       capture_output=True, text=True, timeout=900)
-    assert r.returncode == 0, r.stdout + r.stderr
-    with np.load(path) as z:
-        return {k: z[k] for k in z.files}
+def register_values():
+    """Slot values of k_group_step_e for every case without the fused regulariser: a group's slot values do not depend
+    on the launch, and slices of whole batches keep each batch's BPR count, so the slices concatenated are the values
+    of the whole case."""
+    from torch.profiler import ProfilerActivity, profile
+    for _ in range(3):          # a capture whose kernel records the profiler lost names no kernel of ours: take it again
+        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            run_case(CASES[0], "sparse", slices(N_POS)[0])      # CASES[0] runs on the TMA kernel when whole
+            torch.cuda.synchronize()
+        names = " ".join(e.key for e in prof.key_averages())
+        if "kgrec::" in names:
+            break
+    assert "k_group_step_e" in names and "k_group_step_e_tma" not in names, names
+    out = {}
+    for c in (c for c in CASES if not c[4]):
+        ms = [run_case(c, "sparse", rows)[0] for rows in slices(N_POS)]
+        out[case_id(c)] = {name: np.concatenate([getattr(m, name + "_embeddings").weight.grad._values().cpu().numpy()
+                                                 for m in ms]) for name in ("ent", "rel")}
+    return out
 
 
 @pytest.mark.parametrize("c", CASES, ids=case_id)
@@ -124,12 +131,5 @@ def test_tma_step_matches_register_kernels(c, register_values):
     if not reg:
         for name in ("ent", "rel"):
             got = getattr(ms, name + "_embeddings").weight.grad._values().cpu().numpy()
-            want = register_values[case_id(c) + "/" + name]
+            want = register_values[case_id(c)][name]
             assert got.shape == want.shape and np.array_equal(got.view(np.uint32), want.view(np.uint32)), name
-
-
-if __name__ == "__main__":
-    if len(sys.argv) == 3 and sys.argv[1] == "--dump":
-        dump_register_values(sys.argv[2])
-    else:
-        sys.exit("usage: test_group_step_tma.py --dump OUT.npz")

@@ -153,7 +153,7 @@ def main():
     info_before = gpu_info()
     sizes = [measure(K, int(n), args.min_seconds, dev) for n in args.entities.split(",")]
     out = {"gpu": info_before, "gpu_after": gpu_info(), "shape": {"d": D, "batches": N_BATCHES, "batch": BATCH, "k_neg": K_NEG},
-           "group_step": os.environ.get("KGREC_GROUP_STEP", ""), "sizes": sizes}
+           "sizes": sizes}
     print(json.dumps(out))
 
 
