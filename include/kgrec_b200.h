@@ -509,6 +509,27 @@ int kgrec_eval_rank_count(const kgrec_tables* tables, int model, int side,
                           const float* gold_scores, const int32_t* gold_ids,
                           int32_t* counts, kgrec_stream_t stream);
 
+/* The same count with the filter applied in the kernel: row i adds
+ * #{ e in catalog shard : (score(q_i, e), e) < (gold_scores[i], gold_ids[i]), e not in X_i }
+ * where X_i = excl_ids[excl_ptr[excl_row[i]], excl_ptr[excl_row[i] + 1]) holds ascending GLOBAL ids
+ * (the query's filter set -- train + other eval files -- and its gold set; the gold itself never
+ * counts, the comparison being strict).  Rows that share a query share its exclusion row.  An id is
+ * looked up only when its key is below the gold's.  Shard counts still add.  KG sides only; all
+ * three arrays are required (an empty exclusion is a CSR of empty rows). */
+int kgrec_eval_rank_count_ex(const kgrec_tables* tables, int model, int side,
+                             const void* q, const void* r, int idx_bytes, const float* qvec, int64_t nq,
+                             const float* cat, int64_t cat_ld, int64_t n_cat, int64_t id_base,
+                             const float* gold_scores, const int32_t* gold_ids, int32_t* counts,
+                             const int32_t* excl_row, const int64_t* excl_ptr, const int32_t* excl_ids,
+                             kgrec_stream_t stream);
+
+/* Per-user top-n metrics of the rec side (getRecPerformance, utils/misc.py:213-248): keys [nq, k] from
+ * kgrec_eval_topk (UINT64_MAX places are not part of the list), gold sets as a CSR (gold_ptr [nq+1],
+ * ascending ids).  out [nq, 5] float64 = (f1, precision, recall, hit, ndcg) with precision = hits / list
+ * length and ndcg_at_k method 0 (utils/evaluation.py:41-110); a user without a hit gets zeros. */
+int kgrec_rec_topk_metrics(const uint64_t* keys, int64_t nq, int32_t k, const int64_t* gold_ptr,
+                           const int32_t* gold_ids, double* out, kgrec_stream_t stream);
+
 /* TransR full-catalog evaluation (transR.py:80-128 + projection_transR_pytorch_batch, misc.py:29-33).
  * The reference projects the whole entity table with every query's matrix; queries of one relation
  * share it, so the caller passes the queries SORTED BY RELATION (q / r device arrays, nq of them) with
@@ -534,6 +555,14 @@ int kgrec_transr_eval_rank_count(const kgrec_tables* tables, int side, const voi
                                  const float* cat, int64_t cat_ld, int64_t n_cat, int64_t id_base, float* workspace,
                                  const float* gold_scores, const int32_t* gold_ids, int32_t* counts,
                                  int32_t* status, kgrec_stream_t stream);
+/* kgrec_eval_rank_count_ex on the projected rows; excl_row is indexed in the sorted query order and
+ * holds absolute rows of the exclusion CSR. */
+int kgrec_transr_eval_rank_count_ex(const kgrec_tables* tables, int side, const void* q, const void* r, int idx_bytes,
+                                    int64_t nq, const int64_t* run_begin_host, const int64_t* run_rel_host, int32_t n_runs,
+                                    const float* cat, int64_t cat_ld, int64_t n_cat, int64_t id_base, float* workspace,
+                                    const float* gold_scores, const int32_t* gold_ids, int32_t* counts,
+                                    const int32_t* excl_row, const int64_t* excl_ptr, const int32_t* excl_ids,
+                                    int32_t* status, kgrec_stream_t stream);
 
 /* Soft-preference rec-side evaluation (use_st_gumbel = 0) on augmented rows: with raw logits as
  * mixing weights (transUP.py:108-113) r and w are linear in the logits, so each table row is

@@ -550,7 +550,16 @@ __device__ __noinline__ uint32_t topk_insert_candidates(unsigned mask, uint32_t 
 constexpr int RQ = 8;                         // queries per warp
 
 struct TiledSmem {
-  size_t bars, q, w, gold, tiles, lists, total;
+  size_t bars, q, w, gold, tiles, lists, total, excl;
+};
+
+// Exclusion CSR of the filtered rank count (kgrec_eval_rank_count_ex): row i of the launch skips the global ids
+// ids[ptr[row[i]], ptr[row[i] + 1]) (ascending).  A kernel parameter of its own, behind the existing ones, so the
+// layout of EvalArgs and of the other parameters is that of the unfiltered instantiations.
+struct ExclArgs {
+  const int32_t* row;
+  const int64_t* ptr;
+  const int32_t* ids;
 };
 // Row pitch of a catalog tile in shared memory (floats).  A lane reads one 16-byte chunk of "its" row per step, so
 // 8 consecutive rows must land on 8 different bank groups: true when the row is an odd number of 16-byte units long
@@ -561,7 +570,8 @@ struct TiledSmem {
 __host__ __device__ inline int tile_pitch(int d) { return ((d >> 2) & 1) ? d : d + 4; }
 // ST-Gumbel rec rows: [x (d) | A_k = x . P'_k / 2 (P) | C_k = x . W_k (P) | pad to a multiple of 4]
 __host__ __device__ inline int gumbel_aug_ld(int d, int P) { return (d + 2 * P + 3) & ~3; }
-__host__ __device__ inline TiledSmem tiled_smem_layout(int kind, int mode, int d, int tn, int stages, int k, int warps, int P = 0) {
+__host__ __device__ inline TiledSmem tiled_smem_layout(int kind, int mode, int d, int tn, int stages, int k, int warps, int P = 0,
+                                                       bool excl = false) {
   TiledSmem s{};
   const int TQT = RQ * warps;
   size_t off = 0;
@@ -574,6 +584,9 @@ __host__ __device__ inline TiledSmem tiled_smem_layout(int kind, int mode, int d
     off = (off + 15) & ~static_cast<size_t>(15);
   }
   if (mode == MODE_RANK) { s.gold = off; off += static_cast<size_t>(TQT) * 2 * sizeof(uint32_t); }
+  if (mode == MODE_RANK && excl) {        // per-query exclusion range [lo, hi) of the filtered rank count
+    s.excl = off; off += static_cast<size_t>(TQT) * 2 * sizeof(int64_t);
+  }
   off = (off + 127) & ~static_cast<size_t>(127);
   s.tiles = off; off += static_cast<size_t>(stages) * tn * tile_pitch(kind == KIND_GUMBEL_L2 ? gumbel_aug_ld(d, P) : d) * sizeof(float);
   if (mode == MODE_TOPK) { s.lists = off; off += static_cast<size_t>(TQT) * k * sizeof(uint64_t); }
@@ -581,9 +594,12 @@ __host__ __device__ inline TiledSmem tiled_smem_layout(int kind, int mode, int d
   return s;
 }
 
-template <int KIND, int MODE, bool L1, int RN, int W, bool IDS>
+// EXCL (MODE_RANK only): a row counts only when its key is below the gold key AND its id is not in the query's
+// exclusion row (X); the id is looked up after the key test, so rows ranked behind the gold cost nothing extra.
+template <int KIND, int MODE, bool L1, int RN, int W, bool IDS, bool EXCL = false>
 __global__ void __launch_bounds__(W * 32, 1)
-k_eval_tiled(const EvalArgs A, const int stages, const int64_t units_per_cta) {
+k_eval_tiled(const EvalArgs A, const int stages, const int64_t units_per_cta, const ExclArgs X) {
+  static_assert(!EXCL || MODE == MODE_RANK, "the exclusion CSR belongs to the rank count");
   extern __shared__ __align__(128) unsigned char smem_raw[];
   constexpr int TN = 32 * RN;
   constexpr int TQT = RQ * W;
@@ -591,12 +607,13 @@ k_eval_tiled(const EvalArgs A, const int stages, const int64_t units_per_cta) {
   const kgrec_tables& T = A.T;
   const int d = T.dim;
   const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-  const TiledSmem L = tiled_smem_layout(KIND, MODE, d, TN, stages, A.k, W, T.n_pref);
+  const TiledSmem L = tiled_smem_layout(KIND, MODE, d, TN, stages, A.k, W, T.n_pref, EXCL);
   uint64_t* full = reinterpret_cast<uint64_t*>(smem_raw + L.bars);
   uint64_t* empty = full + 8;
   float* sQ = reinterpret_cast<float*>(smem_raw + L.q);
   [[maybe_unused]] float* sW = reinterpret_cast<float*>(smem_raw + L.w);
   [[maybe_unused]] uint32_t* sGold = reinterpret_cast<uint32_t*>(smem_raw + L.gold);
+  [[maybe_unused]] int64_t* sExcl = reinterpret_cast<int64_t*>(smem_raw + L.excl);
   float* tiles = reinterpret_cast<float*>(smem_raw + L.tiles);
   const int rf = (KIND == KIND_GUMBEL_L2) ? gumbel_aug_ld(d, T.n_pref) : d;   // floats of a catalog row that travel
   const int pitch = tile_pitch(rf);
@@ -648,6 +665,7 @@ k_eval_tiled(const EvalArgs A, const int stages, const int64_t units_per_cta) {
   const float* cq = sQ + wid * RQ * d;
   [[maybe_unused]] const float* wq = sW + wid * RQ * d;
   [[maybe_unused]] const uint32_t* gq = sGold + wid * RQ * 2;
+  [[maybe_unused]] const int64_t* xq = sExcl + wid * RQ * 2;
   const int nk4 = d >> 2;
   // Every row is walked in the same dimension order, so a (query, row) score is bit-identical wherever the row
   // sits (tile, lane, shard, gathered sub-catalog).
@@ -704,6 +722,18 @@ k_eval_tiled(const EvalArgs A, const int stages, const int64_t units_per_cta) {
         if (lane == 0) {
           sGold[(wid * RQ + qi) * 2] = q < A.nq ? __float_as_uint(__ldg(A.gold_scores + q)) : 0u;
           sGold[(wid * RQ + qi) * 2 + 1] = q < A.nq ? static_cast<uint32_t>(__ldg(A.gold_ids + q)) : 0u;
+        }
+        if constexpr (EXCL) {
+          if (lane == 1) {
+            int64_t lo = 0, hi = 0;
+            if (q < A.nq) {
+              const int64_t row = __ldg(X.row + q);
+              lo = __ldg(X.ptr + row);
+              hi = __ldg(X.ptr + row + 1);
+            }
+            sExcl[(wid * RQ + qi) * 2] = lo;
+            sExcl[(wid * RQ + qi) * 2 + 1] = hi;
+          }
         }
       }
     }
@@ -922,7 +952,12 @@ k_eval_tiled(const EvalArgs A, const int stages, const int64_t units_per_cta) {
         } else if constexpr (MODE == MODE_RANK) {
           const uint32_t id = static_cast<uint32_t>(A.id_base + n_local);
           const uint32_t gh = gq[qi * 2], gi = gq[qi * 2 + 1];
-          if (valid && (sb < gh || (sb == gh && id < gi))) ++cnt[qi];
+          if constexpr (EXCL) {
+            if (valid && (sb < gh || (sb == gh && id < gi)) && !filtered(X.ids, xq[qi * 2], xq[qi * 2 + 1], static_cast<int32_t>(id)))
+              ++cnt[qi];
+          } else {
+            if (valid && (sb < gh || (sb == gh && id < gi))) ++cnt[qi];
+          }
         } else {
           const unsigned mask = __ballot_sync(FULL, valid && sb <= thr_hi[qi]);
           if (mask) {                            // rare once the lists have warmed up
@@ -1324,7 +1359,7 @@ static int eval_rotate() {
 }
 
 static int eval_plan(const kgrec_tables* T, int model, int side, int mode, const float* cat, int64_t cat_ld,
-                     int64_t nq, int64_t n_cat, int k, bool have_qvec, EvalArgs* A, EvalPlan* pl) {
+                     int64_t nq, int64_t n_cat, int k, bool have_qvec, EvalArgs* A, EvalPlan* pl, bool excl = false) {
   if (!T) { set_error("tables is NULL"); return KGREC_ERR_INVALID; }
   if (!cat || n_cat <= 0 || nq <= 0) { set_error("empty catalog / query set"); return KGREC_ERR_INVALID; }
   const int d = T->dim;
@@ -1423,10 +1458,10 @@ static int eval_plan(const kgrec_tables* T, int model, int side, int mode, const
     pl->rn = (pl->kind == KIND_DIST ? 4 : 2) / (wide ? 2 : 1);
     const int tn_t = 32 * pl->rn;
     int stages = 4;
-    while (stages > 2 && tiled_smem_layout(pl->kind, mode, d, tn_t, stages, k, pl->warps).total > 210 * 1024) --stages;
+    while (stages > 2 && tiled_smem_layout(pl->kind, mode, d, tn_t, stages, k, pl->warps, 0, excl).total > 210 * 1024) --stages;
     pl->stages = stages;
     pl->tn = tn_t;
-    pl->smem = tiled_smem_layout(pl->kind, mode, d, tn_t, stages, k, pl->warps).total;
+    pl->smem = tiled_smem_layout(pl->kind, mode, d, tn_t, stages, k, pl->warps, 0, excl).total;
     if (pl->smem > 225 * 1024) { set_error("eval: shared-memory budget exceeded (%zu bytes)", pl->smem); return KGREC_ERR_UNSUPPORTED; }
     const int64_t n_tiles_t = (n_cat + tn_t - 1) / tn_t;
     const int tqt = RQ * pl->warps;
@@ -1468,7 +1503,7 @@ static int eval_plan(const kgrec_tables* T, int model, int side, int mode, const
 }
 
 template <int MODE>
-static int launch_eval(const EvalArgs& A, const EvalPlan& pl, cudaStream_t st) {
+static int launch_eval(const EvalArgs& A, const EvalPlan& pl, cudaStream_t st, const ExclArgs& X = ExclArgs{}) {
   const dim3 grid(static_cast<unsigned>(pl.n_qtiles), static_cast<unsigned>(pl.n_splits));
   if (pl.soft_aug) {
     if constexpr (MODE == MODE_RANK) {
@@ -1489,8 +1524,11 @@ static int launch_eval(const EvalArgs& A, const EvalPlan& pl, cudaStream_t st) {
     if constexpr (MODE == MODE_FULL) {                                                                        \
       if (A.cat_ids) kern = A.T.l1 ? k_eval_tiled<KINDV, MODE, true, RNV, WV, true> : k_eval_tiled<KINDV, MODE, false, RNV, WV, true>; \
     }                                                                                                         \
+    if constexpr (MODE == MODE_RANK) {                                                                        \
+      if (X.row) kern = A.T.l1 ? k_eval_tiled<KINDV, MODE, true, RNV, WV, false, true> : k_eval_tiled<KINDV, MODE, false, RNV, WV, false, true>; \
+    }                                                                                                         \
     KGREC_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(pl.smem))); \
-    kern<<<pl.grid, WV * 32, pl.smem, st>>>(A, pl.stages, pl.units_per_cta);                                  \
+    kern<<<pl.grid, WV * 32, pl.smem, st>>>(A, pl.stages, pl.units_per_cta, X);                               \
   }
     if (pl.kind == KIND_DIST) { if (pl.warps == 16) KGREC_TILED_CASE(KIND_DIST, 4, 16) else KGREC_TILED_CASE(KIND_DIST, 2, 8) }
     else if (pl.kind == KIND_GUMBEL_L2) {
@@ -1602,23 +1640,106 @@ extern "C" int kgrec_merge_topk(const uint64_t* in_keys, int32_t n_lists, int64_
   return KGREC_OK;
 }
 
-extern "C" int kgrec_eval_rank_count(const kgrec_tables* tables, int model, int side, const void* q, const void* r,
-                                     int idx_bytes, const float* qvec, int64_t nq, const float* cat, int64_t cat_ld,
-                                     int64_t n_cat, int64_t id_base, const float* gold_scores, const int32_t* gold_ids,
-                                     int32_t* counts, kgrec_stream_t stream) {
+// kgrec_eval_rank_count (X == NULL) and kgrec_eval_rank_count_ex (X = the exclusion CSR)
+static int rank_count(const kgrec_tables* tables, int model, int side, const void* q, const void* r, int idx_bytes,
+                      const float* qvec, int64_t nq, const float* cat, int64_t cat_ld, int64_t n_cat, int64_t id_base,
+                      const float* gold_scores, const int32_t* gold_ids, int32_t* counts, const ExclArgs* X,
+                      kgrec_stream_t stream) {
   EvalArgs A{};
   EvalPlan pl{};
-  int rc = eval_plan(tables, model, side, MODE_RANK, cat, cat_ld, nq, n_cat, 0, qvec != nullptr, &A, &pl);
+  int rc = eval_plan(tables, model, side, MODE_RANK, cat, cat_ld, nq, n_cat, 0, qvec != nullptr, &A, &pl, X != nullptr);
   if (rc) return rc;
   if (!gold_scores || !gold_ids || !counts) { set_error("rank_count: NULL argument"); return KGREC_ERR_INVALID; }
   if (!qvec && (!q || (side != KGREC_SIDE_REC && !r))) { set_error("query ids are NULL"); return KGREC_ERR_INVALID; }
   if (!qvec && idx_bytes != 4 && idx_bytes != 8) { set_error("idx_bytes must be 4 or 8"); return KGREC_ERR_INVALID; }
   A.q = q; A.r = r; A.is64 = idx_bytes == 8; A.qvec = qvec;
   if (id_base < 0 || id_base + n_cat > 0xffffffffll) { set_error("catalog ids must fit 32 bits"); return KGREC_ERR_INVALID; }
+  if (X) {
+    if (!X->row || !X->ptr || !X->ids) { set_error("rank_count_ex: exclusion CSR (excl_row / excl_ptr / excl_ids) has a NULL array"); return KGREC_ERR_INVALID; }
+    if ((reinterpret_cast<uintptr_t>(X->row) & 3u) || (reinterpret_cast<uintptr_t>(X->ptr) & 7u) || (reinterpret_cast<uintptr_t>(X->ids) & 3u)) {
+      set_error("rank_count_ex: exclusion CSR arrays are not aligned to their element size");
+      return KGREC_ERR_INVALID;
+    }
+    if (!pl.tiled) { set_error("rank_count_ex: filtered rank counts are built for the KG sides"); return KGREC_ERR_UNSUPPORTED; }
+  }
   A.qvec_ld = 2 * static_cast<int64_t>(tables->dim);
   A.id_base = id_base; A.seed = 0;
   A.gold_scores = gold_scores; A.gold_ids = gold_ids; A.counts = counts;
-  return launch_eval<MODE_RANK>(A, pl, static_cast<cudaStream_t>(stream));
+  return launch_eval<MODE_RANK>(A, pl, static_cast<cudaStream_t>(stream), X ? *X : ExclArgs{});
+}
+
+extern "C" int kgrec_eval_rank_count(const kgrec_tables* tables, int model, int side, const void* q, const void* r,
+                                     int idx_bytes, const float* qvec, int64_t nq, const float* cat, int64_t cat_ld,
+                                     int64_t n_cat, int64_t id_base, const float* gold_scores, const int32_t* gold_ids,
+                                     int32_t* counts, kgrec_stream_t stream) {
+  return rank_count(tables, model, side, q, r, idx_bytes, qvec, nq, cat, cat_ld, n_cat, id_base, gold_scores, gold_ids, counts,
+                    nullptr, stream);
+}
+
+extern "C" int kgrec_eval_rank_count_ex(const kgrec_tables* tables, int model, int side, const void* q, const void* r,
+                                        int idx_bytes, const float* qvec, int64_t nq, const float* cat, int64_t cat_ld,
+                                        int64_t n_cat, int64_t id_base, const float* gold_scores, const int32_t* gold_ids,
+                                        int32_t* counts, const int32_t* excl_row, const int64_t* excl_ptr,
+                                        const int32_t* excl_ids, kgrec_stream_t stream) {
+  const ExclArgs X{excl_row, excl_ptr, excl_ids};
+  return rank_count(tables, model, side, q, r, idx_bytes, qvec, nq, cat, cat_ld, n_cat, id_base, gold_scores, gold_ids, counts,
+                    &X, stream);
+}
+
+// Per-user top-n metrics of the rec side (getRecPerformance, utils/misc.py:213-248; evaluation.rec_metrics_from_topk):
+// one warp per user walks its key list in order; lanes test 32 places at a time against the ascending gold ids.
+__global__ void __launch_bounds__(256)
+k_rec_topk_metrics(const uint64_t* __restrict__ keys, int64_t nq, int k, const int64_t* __restrict__ gold_ptr,
+                   const int32_t* __restrict__ gold_ids, double* __restrict__ out) {
+  const int lane = threadIdx.x & 31;
+  for (int64_t q = static_cast<int64_t>(blockIdx.x) * 8 + (threadIdx.x >> 5); q < nq; q += static_cast<int64_t>(gridDim.x) * 8) {
+    const int64_t g_lo = __ldg(gold_ptr + q), g_hi = __ldg(gold_ptr + q + 1);
+    int n_list = 0, n_hit = 0;                 // warp-uniform
+    double dcg = 0.0;
+    for (int base = 0; base < k; base += 32) {
+      const int j = base + lane;
+      const uint64_t key = j < k ? __ldg(keys + q * k + j) : KEY_INF;
+      const bool listed = key != KEY_INF;      // empty places are not part of the list
+      const bool hit = listed && filtered(gold_ids, g_lo, g_hi, static_cast<int32_t>(key & 0xffffffffu));
+      const unsigned lm = __ballot_sync(FULL, listed);
+      unsigned hm = __ballot_sync(FULL, hit);
+      while (hm) {                             // hits in list order; ndcg_at_k method 0: weights 1, 1, 1/log2(3), ...
+        const int src = __ffs(hm) - 1;
+        hm &= hm - 1;
+        const int pos = n_list + __popc(lm & ((1u << src) - 1u));
+        dcg += pos == 0 ? 1.0 : 1.0 / log2(pos + 1.0);
+        ++n_hit;
+      }
+      n_list += __popc(lm);
+    }
+    if (lane == 0) {
+      double* o = out + q * 5;
+      if (n_hit == 0) {
+        for (int i = 0; i < 5; ++i) o[i] = 0.0;
+      } else {
+        double idcg = 1.0;
+        for (int pos = 1; pos < n_hit; ++pos) idcg += 1.0 / log2(pos + 1.0);
+        const double p = static_cast<double>(n_hit) / n_list, r = static_cast<double>(n_hit) / static_cast<double>(g_hi - g_lo);
+        o[0] = 2.0 * p * r / (p + r);
+        o[1] = p;
+        o[2] = r;
+        o[3] = 1.0;
+        o[4] = dcg / idcg;
+      }
+    }
+  }
+}
+
+extern "C" int kgrec_rec_topk_metrics(const uint64_t* keys, int64_t nq, int32_t k, const int64_t* gold_ptr,
+                                      const int32_t* gold_ids, double* out, kgrec_stream_t stream) {
+  if (nq < 0 || k < 1) { set_error("rec_topk_metrics: nq must be >= 0 and k >= 1"); return KGREC_ERR_INVALID; }
+  if (nq == 0) return KGREC_OK;
+  if (!keys || !gold_ptr || !gold_ids || !out) { set_error("rec_topk_metrics: NULL argument"); return KGREC_ERR_INVALID; }
+  const int64_t ctas = (nq + 7) / 8, cap = static_cast<int64_t>(sm_count()) * 16;
+  k_rec_topk_metrics<<<static_cast<unsigned>(ctas < cap ? ctas : cap), 256, 0, static_cast<cudaStream_t>(stream)>>>(
+      keys, nq, k, gold_ptr, gold_ids, out);
+  KGREC_CUDA_OK(cudaGetLastError());
+  return KGREC_OK;
 }
 
 extern "C" int kgrec_ktup_item_table(const kgrec_tables* tables, int64_t item_begin, int64_t n_items, float* out,

@@ -159,6 +159,12 @@ _SIGNATURES = {
     "kgrec_eval_rank_count": (C.c_int, [C.POINTER(Tables), C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int,
                                         C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_int64, C.c_int64,
                                         C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "kgrec_eval_rank_count_ex": (C.c_int, [C.POINTER(Tables), C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int,
+                                           C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_int64, C.c_int64,
+                                           C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                           C.c_void_p]),
+    "kgrec_rec_topk_metrics": (C.c_int, [C.c_void_p, C.c_int64, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
+                                         C.c_void_p]),
     "kgrec_transr_workspace_floats": (C.c_int64, [C.c_int64, C.c_int64, C.c_int32]),
     "kgrec_transr_eval_scores": (C.c_int, [C.POINTER(Tables), C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_int64,
                                            C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_int64, C.c_int64, C.c_int64,
@@ -170,6 +176,10 @@ _SIGNATURES = {
     "kgrec_transr_eval_rank_count": (C.c_int, [C.POINTER(Tables), C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_int64,
                                                C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_int64, C.c_int64, C.c_int64,
                                                C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "kgrec_transr_eval_rank_count_ex": (C.c_int, [C.POINTER(Tables), C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_int64,
+                                                  C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_int64, C.c_int64,
+                                                  C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                                  C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "kgrec_gumbel_aug_ld": (C.c_int32, [C.c_int32, C.c_int32]),
     "kgrec_gumbel_aug_supported": (C.c_int32, [C.c_int32, C.c_int32, C.c_int32]),
     "kgrec_gumbel_aug_rows": (C.c_int, [C.POINTER(Tables), C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_int64, C.c_int64,

@@ -13,10 +13,18 @@ Semantics restated from the reference (ties broken by (score, id), see oracle/kg
   KG  : for every gold id g of a query, rank(g) = #{ e not in filter, not gold : e sorts before g };
         hit = rank < topn (misc.py:125-146).  A gold id that is itself in the filter set is never
         reached by the reference's walk and is skipped here too.
+
+evaluate_rec / evaluate_kg rebuild the per-query filter sets on the host at every call.  KGEvaluator and
+RecEvaluator do that host work once, for a fixed set of eval / filter dicts, and then evaluate the current
+tables with device work only (the loop-with-validation form, INTEGRATION section 4).
 """
+import ctypes as C
+import itertools
+
 import numpy as np
 import torch
 
+from . import _lib
 from . import evaluation as KE
 from . import functional as KF
 
@@ -125,3 +133,281 @@ def evaluate_kg(model, eval_head_dict, eval_tail_dict, all_head_dicts=None, all_
     tot = max(1, n_h + n_t)
     return (float(h[0] * n_h + t[0] * n_t) / tot, float(h[1] * n_h + t[1] * n_t) / tot,
             (float(h[0]), float(h[1])), (float(t[0]), float(t[1])))
+
+
+# ---- evaluators: host work once per (eval dicts, filter dicts), device work per evaluation ---------------
+def _flatten_sets(keys, dct):
+    """(lengths [len(keys)], ids) of dct[key] for every key, each set in its own iteration order."""
+    sets = [dct[k] for k in keys]
+    lens = np.fromiter((len(s) for s in sets), dtype=np.int64, count=len(sets))
+    ids = np.fromiter(itertools.chain.from_iterable(sets), dtype=np.int64, count=int(lens.sum()))
+    return lens, ids
+
+
+def _csr(codes, n_rows, width):
+    """Sorted (row * width + id) codes -> (ptr int64 [n_rows + 1], ids int64)."""
+    ptr = np.zeros(n_rows + 1, dtype=np.int64)
+    np.cumsum(np.bincount(codes // width, minlength=n_rows), out=ptr[1:])
+    return ptr, codes % width
+
+
+def side_arrays(keys, eval_dict, all_dicts, drop_filtered_gold):
+    """Host arrays of one evaluation side (query keys = the eval dict's keys with a non-empty gold set).
+
+    Returns a dict of int64 numpy arrays:
+      pair_q, pair_gold  one entry per (query index, gold id), queries in `keys` order and each gold set in
+                         its iteration order -- the order evaluate_kg / evaluate_rec visit them; with
+                         drop_filtered_gold, golds inside the query's filter set are left out (the reference's
+                         walk never reaches them, misc.py:125-146)
+      filt_ptr, filt_ids the filter CSR: per query the ascending union over all_dicts of dict[key]
+      excl_ptr, excl_ids the exclusion CSR: per query the ascending union of its filter and gold sets
+      gold_ptr, gold_ids the gold CSR: per query its ascending gold set
+    """
+    nq = len(keys)
+    g_len, g_ids = _flatten_sets(keys, eval_dict)
+    g_q = np.repeat(np.arange(nq, dtype=np.int64), g_len)
+    f_q, f_ids = [np.zeros(0, np.int64)], [np.zeros(0, np.int64)]
+    for d in all_dicts or ():
+        present = [i for i, k in enumerate(keys) if k in d]
+        lens, ids = _flatten_sets([keys[i] for i in present], d)
+        f_q.append(np.repeat(np.asarray(present, dtype=np.int64), lens))
+        f_ids.append(ids)
+    f_q, f_ids = np.concatenate(f_q), np.concatenate(f_ids)
+    if (g_ids.size and g_ids.min() < 0) or (f_ids.size and f_ids.min() < 0):
+        raise ValueError("kgrec_b200: negative ids in the eval / filter dicts")
+    width = 1 + int(max(g_ids.max(initial=0), f_ids.max(initial=0)))
+    f_code = np.unique(f_q * width + f_ids)
+    g_code = g_q * width + g_ids
+    keep = ~np.isin(g_code, f_code) if drop_filtered_gold else np.ones(g_code.size, dtype=bool)
+    out = {"pair_q": g_q[keep], "pair_gold": g_ids[keep]}
+    out["filt_ptr"], out["filt_ids"] = _csr(f_code, nq, width)
+    out["excl_ptr"], out["excl_ids"] = _csr(np.union1d(f_code, g_code), nq, width)
+    out["gold_ptr"], out["gold_ids"] = _csr(np.sort(g_code), nq, width)
+    return out
+
+
+def _dev_ids(a, dev, dtype):
+    """Host id array -> device tensor; an empty CSR id array still gets one (never read) element."""
+    a = np.asarray(a)
+    if a.size and (a.min() < np.iinfo(np.int32).min or a.max() > np.iinfo(np.int32).max) and dtype == torch.int32:
+        raise ValueError("kgrec_b200: ids must fit 32 bits")
+    return torch.as_tensor(a if a.size else np.zeros(1, a.dtype), device=dev).to(dtype).contiguous()
+
+
+class _KGSide:
+    """Device arrays of one KG side.  TransR keeps its pairs sorted by relation (kgrec_transr_eval_* take the queries
+    of one relation as one run) and maps the ranks back to the driver's order with `inv`."""
+
+    def __init__(self, model, side, eval_dict, all_dicts, chunk, transr):
+        dev = model.device
+        self.sd = _lib.SIDE_HEAD if side == "head" else _lib.SIDE_TAIL
+        keys = [k for k, gold in eval_dict.items() if len(gold) > 0]
+        a = side_arrays(keys, eval_dict, all_dicts, drop_filtered_gold=True)
+        kq = np.fromiter((k[0] for k in keys), dtype=np.int64, count=len(keys))
+        kr = np.fromiter((k[1] for k in keys), dtype=np.int64, count=len(keys))
+        q, r, gold, row = kq[a["pair_q"]], kr[a["pair_q"]], a["pair_gold"], a["pair_q"]
+        n_ent, n_rel = model.ent_embeddings.weight.shape[0], model.rel_embeddings.weight.shape[0]
+        for name, ids, bound in (("query", q, n_ent), ("relation", r, n_rel), ("gold", gold, n_ent)):
+            if ids.size and (ids.min() < 0 or ids.max() >= bound):
+                raise IndexError("kgrec_b200: a %s id of the %s eval dict is out of range for its table" % (name, side))
+        self.n = int(q.size)
+        self.inv = None
+        if transr and self.n:
+            order = np.argsort(r, kind="stable")
+            q, r, gold, row = q[order], r[order], gold[order], row[order]
+            inv = np.empty_like(order)
+            inv[order] = np.arange(order.size)
+            self.inv = torch.as_tensor(inv, device=dev)
+            cut = np.flatnonzero(np.diff(r)) + 1
+            self.run_begin = torch.as_tensor(np.concatenate([[0], cut, [self.n]]).astype(np.int64))   # host arrays
+            self.run_rel = torch.as_tensor(r[np.concatenate([[0], cut])].astype(np.int64))
+            # gold-score chunks of the sorted pairs, each with the run boundaries inside it
+            self.chunks = []
+            for lo in range(0, self.n, chunk):
+                hi = min(self.n, lo + chunk)
+                b = np.concatenate([[lo], cut[(cut > lo) & (cut < hi)], [hi]]).astype(np.int64)
+                self.chunks.append((lo, hi, torch.as_tensor(b - lo), torch.as_tensor(r[b[:-1]].astype(np.int64))))
+        self.q = torch.as_tensor(q, device=dev)
+        self.r = torch.as_tensor(r, device=dev)
+        self.gold = torch.as_tensor(gold, device=dev)
+        self.gold32 = _dev_ids(gold, dev, torch.int32)
+        self.excl_row = _dev_ids(row, dev, torch.int32)
+        self.excl_ptr = torch.as_tensor(a["excl_ptr"], device=dev)
+        self.excl_ids = _dev_ids(a["excl_ids"], dev, torch.int32)
+        self.pairs = (kq[a["pair_q"]], kr[a["pair_q"]], a["pair_gold"])    # host copy, driver order
+
+
+class KGEvaluator:
+    """Filtered KG validation (hit@topn and mean rank of both sides, as evaluate_kg) with the host work done once.
+
+    The constructor turns the eval and filter dicts into device arrays: one row per (query, gold) pair, the query's
+    exclusion CSR (filter set + gold set, ascending) and, for TransR, the relation-sorted order with its runs.
+    run() then scores the current tables with device work only:
+      1. gold scores by the catalog pass's own arithmetic (the gathered gold rows as an id-tagged sub-catalog, in
+         chunks of `chunk` pairs; the diagonal of each [chunk, chunk] block), bit-identical to what the count compares;
+      2. one filtered rank-count pass per side (kgrec_eval_rank_count_ex / kgrec_transr_eval_rank_count_ex);
+      3. hit and rank sums as a [4] float64 device tensor.
+    result(m) reads it back (the one synchronisation) and returns evaluate_kg's tuple.
+    Models: TransE, TransH, TransR, and jTransUP's KG branch (TransH kernels on the KTUP tables, padding row included).
+    """
+
+    def __init__(self, model, eval_head_dict, eval_tail_dict, all_head_dicts=None, all_tail_dicts=None, topn=10, chunk=512):
+        self.model = model
+        self.topn = int(topn)
+        self.chunk = int(chunk)
+        dev = model._require_cuda()
+        self._transr = model.MODEL == _lib.TRANSR
+        self._kg = _lib.TRANSH if model.MODEL == _lib.KTUP else model.MODEL
+        self.sides = (_KGSide(model, "head", eval_head_dict, all_head_dicts, self.chunk, self._transr),
+                      _KGSide(model, "tail", eval_tail_dict, all_tail_dicts, self.chunk, self._transr))
+        n_cat, d = model.ent_embeddings.weight.shape
+        n_max = max(s.n for s in self.sides)
+        c = min(self.chunk, max(1, n_max))
+        self._blk = torch.empty((c, c), dtype=torch.float32, device=dev)         # gold-score blocks
+        self._ws = self._ws_gold = None
+        if self._transr:
+            lib = _lib.load()
+            self._ws = torch.empty(int(lib.kgrec_transr_workspace_floats(max(1, n_max), n_cat, d)), dtype=torch.float32, device=dev)
+            self._ws_gold = torch.empty(int(lib.kgrec_transr_workspace_floats(c, c, d)), dtype=torch.float32, device=dev)
+
+    def _tables(self):
+        m = self.model
+        if self._transr:
+            return KF.make_tables(m._weights(), m.embedding_size, m.L1_flag)
+        return KF.make_tables(m._weights(), m.embedding_size, m.L1_flag, m.use_st_gumbel, m._item2ent)
+
+    def _gold_scores(self, T, s, catalog):
+        lib = _lib.load()
+        rows = catalog.index_select(0, s.gold)
+        gs = torch.empty(s.n, dtype=torch.float32, device=catalog.device)
+        stream = KF._stream()
+        if self._transr:
+            status = self.model._status_buf(catalog.device)
+            for lo, hi, begin, rel in s.chunks:
+                n = hi - lo
+                _lib.check(lib.kgrec_transr_eval_scores(
+                    C.byref(T), s.sd, KF._ptr(s.q[lo:hi]), KF._ptr(s.r[lo:hi]), 8, n, C.c_void_p(begin.data_ptr()),
+                    C.c_void_p(rel.data_ptr()), rel.numel(), KF._ptr(rows[lo:hi]), rows.stride(0), n, 0,
+                    KF._ptr(s.gold32[lo:hi]), KF._ptr(self._ws_gold), KF._ptr(self._blk), self._blk.stride(0),
+                    KF._ptr(status), stream))
+                gs[lo:hi].copy_(self._blk[:n, :n].diagonal())
+        else:
+            for lo in range(0, s.n, self.chunk):
+                hi = min(s.n, lo + self.chunk)
+                KE.run(T, self._kg, s.sd, s.q[lo:hi], s.r[lo:hi], "scores", rows[lo:hi], cat_ids=s.gold32[lo:hi],
+                       out=self._blk[:hi - lo, :hi - lo])
+                gs[lo:hi].copy_(self._blk[:hi - lo, :hi - lo].diagonal())
+        return gs
+
+    def ranks(self):
+        """Filtered rank of every (query, gold) pair of the head and the tail side under the current tables: two
+        int32 device tensors in the order evaluate_kg visits the pairs (`sides[i].pairs` holds them on the host)."""
+        m = self.model
+        dev = m._require_cuda()
+        lib = _lib.load()
+        T = self._tables()
+        catalog = m.ent_embeddings.weight.detach()
+        n_cat = catalog.shape[0]
+        out = []
+        for s in self.sides:
+            counts = torch.zeros(s.n, dtype=torch.int32, device=dev)
+            if s.n:
+                gs = self._gold_scores(T, s, catalog)
+                if self._transr:
+                    _lib.check(lib.kgrec_transr_eval_rank_count_ex(
+                        C.byref(T), s.sd, KF._ptr(s.q), KF._ptr(s.r), 8, s.n, C.c_void_p(s.run_begin.data_ptr()),
+                        C.c_void_p(s.run_rel.data_ptr()), s.run_rel.numel(), KF._ptr(catalog), catalog.stride(0), n_cat, 0,
+                        KF._ptr(self._ws), KF._ptr(gs), KF._ptr(s.gold32), KF._ptr(counts), KF._ptr(s.excl_row),
+                        KF._ptr(s.excl_ptr), KF._ptr(s.excl_ids), KF._ptr(m._status_buf(dev)), KF._stream()))
+                    counts = counts.index_select(0, s.inv)
+                else:
+                    _lib.check(lib.kgrec_eval_rank_count_ex(
+                        C.byref(T), self._kg, s.sd, KF._ptr(s.q), KF._ptr(s.r), 8, None, s.n, KF._ptr(catalog),
+                        catalog.stride(0), n_cat, 0, KF._ptr(gs), KF._ptr(s.gold32), KF._ptr(counts), KF._ptr(s.excl_row),
+                        KF._ptr(s.excl_ptr), KF._ptr(s.excl_ids), KF._stream()))
+                    KF.count_launches(1)
+            out.append(counts)
+        return tuple(out)
+
+    def run(self):
+        """[4] float64 device tensor: (head hits, head rank sum, tail hits, tail rank sum), queued on the current
+        stream with no host synchronisation."""
+        parts = []
+        for c in self.ranks():
+            c = c.to(torch.int64)
+            parts += [(c < self.topn).sum(), c.sum()]
+        return torch.stack(parts).to(torch.float64)
+
+    def result(self, m):
+        """(avg_hit, avg_mean_rank, (head hit, head rank), (tail hit, tail rank)) -- evaluate_kg's tuple, bit for bit."""
+        hh, hr, th, tr = m.tolist()
+        n_h, n_t = self.sides[0].n, self.sides[1].n
+        h = (hh / n_h, hr / n_h) if n_h else (0.0, 0.0)
+        t = (th / n_t, tr / n_t) if n_t else (0.0, 0.0)
+        tot = max(1, n_h + n_t)
+        return (float(h[0] * n_h + t[0] * n_t) / tot, float(h[1] * n_h + t[1] * n_t) / tot, (h[0], h[1]), (t[0], t[1]))
+
+
+class RecEvaluator:
+    """Rec-side validation (mean f1 / precision / recall / hit / NDCG@topn, as evaluate_rec) with the host work done
+    once: the users with a non-empty gold set, their filter CSR and their gold CSR live on the device.  run() builds the
+    catalog of the current tables (TUP soft / ST-Gumbel augmented rows, KTUP's item + entity table), takes the
+    filtered top-n of every user in one call and reduces them on the device (kgrec_rec_topk_metrics); result(m) reads
+    back five numbers.  ST-Gumbel draws come from `seed` (passed by value; one draw per (user position, item,
+    preference)) or from explicit uniforms `gumbel_u` [n_users, n_items, P].
+    """
+
+    def __init__(self, model, eval_dict, all_dicts=None, topn=10):
+        self.model = model
+        self.topn = int(topn)
+        dev = model._require_cuda()
+        users = [u for u, gold in eval_dict.items() if len(gold) > 0]
+        a = side_arrays(users, eval_dict, all_dicts, drop_filtered_gold=False)
+        u = np.asarray(users, dtype=np.int64)
+        if u.size and (u.min() < 0 or u.max() >= model.user_embeddings.weight.shape[0]):
+            raise IndexError("kgrec_b200: a user id of the eval dict is out of range for its table")
+        self.n = int(u.size)
+        self.users = torch.as_tensor(u, device=dev)
+        self.filter_csr = (torch.as_tensor(a["filt_ptr"], device=dev), _dev_ids(a["filt_ids"], dev, torch.int32))
+        self.gold_ptr = torch.as_tensor(a["gold_ptr"], device=dev)
+        self.gold_ids = _dev_ids(a["gold_ids"], dev, torch.int32)
+
+    def topk(self, seed=0, gumbel_u=None):
+        """[n_users, topn] filtered top-n keys of the current tables (the dispatch of RecModelBase._rec_call)."""
+        m, k = self.model, self.topn
+        user_rows = m.user_embeddings.weight.detach()
+        kw = dict(k=k, filter_csr=self.filter_csr)
+        if m._gumbel_aug_ok(k):
+            cat = m.gumbel_catalog()
+            qrows = m._gumbel_rows(user_rows, ids=self.users, with_consts=True)
+            return m._eval(m.MODEL, _lib.SIDE_REC, None, None, "topk", catalog=cat, qvec=qrows, gumbel_u=gumbel_u, seed=seed, **kw)
+        if not m.use_st_gumbel and m.embedding_size % 4 == 0 and m.embedding_size <= 256:
+            cat = m.soft_catalog()
+            qrows = m._aug_rows(user_rows, True, ids=self.users)
+            return m._eval(m.MODEL, _lib.SIDE_REC, None, None, "topk", catalog=cat, qvec=qrows, **kw)
+        return m._eval(m.MODEL, _lib.SIDE_REC, self.users, None, "topk", catalog=m._rec_catalog(), gumbel_u=gumbel_u,
+                       seed=seed if m.use_st_gumbel else 0, **kw)
+
+    def per_user(self, seed=0, gumbel_u=None):
+        """[n_users, 5] float64 device tensor: (f1, p, r, hit, ndcg) per user, users in eval_dict order."""
+        dev = self.model._require_cuda()
+        out = torch.empty((self.n, 5), dtype=torch.float64, device=dev)
+        if self.n:
+            keys = self.topk(seed, gumbel_u)
+            _lib.check(_lib.load().kgrec_rec_topk_metrics(KF._ptr(keys), self.n, self.topn, KF._ptr(self.gold_ptr),
+                                                          KF._ptr(self.gold_ids), KF._ptr(out), KF._stream()))
+            KF.count_launches(1)
+        return out
+
+    def run(self, seed=0, gumbel_u=None):
+        """[5] float64 device tensor of the per-user sums, queued on the current stream with no host synchronisation
+        (the hit sum is an exact count; result() divides on the host, as evaluate_rec's mean does)."""
+        if not self.n:
+            return torch.zeros(5, dtype=torch.float64, device=self.model._require_cuda())
+        return self.per_user(seed, gumbel_u).sum(0)
+
+    def result(self, m):
+        """(f1, precision, recall, hit, ndcg) -- evaluate_rec's tuple."""
+        if not self.n:
+            return (0.0,) * 5
+        return tuple(x / self.n for x in m.tolist())
