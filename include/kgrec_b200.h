@@ -572,6 +572,13 @@ int kgrec_transr_eval_rank_count_ex(const kgrec_tables* tables, int side, const 
  * table, or the kgrec_ktup_item_table output), then call kgrec_eval_scores / kgrec_eval_topk
  * with side = KGREC_SIDE_REC, qvec = the augmented query rows and cat = the augmented catalog. */
 int32_t kgrec_pref_aug_ld(int32_t dim);
+/* 1 when the augmented soft-preference kernel fits this (embedding_size, top-k [0 = score matrix]); where it does
+ * not (148 <= d <= 256, or top-k >= 62 at d = 128), evaluate with user / item ids on the plain path instead. */
+int32_t kgrec_pref_aug_supported(int32_t dim, int32_t k);
+/* 1 when the plain rec-side path (user / item ids, no augmented rows) fits this (embedding_size, preference_total,
+ * use_st_gumbel, top-k [0 = score matrix]).  It stages both preference tables whole, so it has a limit in
+ * preference_total x embedding_size: at d = 256 and top-k 128, soft preferences fit up to preference_total 25. */
+int32_t kgrec_pref_eval_supported(int32_t dim, int32_t n_pref, int32_t use_gumbel, int32_t k);
 int kgrec_pref_aug_rows(const kgrec_tables* tables, int model, int is_query,
                         const void* ids, int idx_bytes, const float* rows, int64_t row_ld, int64_t n,
                         float* out, int64_t ld_out, kgrec_stream_t stream);

@@ -1353,6 +1353,14 @@ struct EvalPlan {
   int64_t units_per_cta;
 };
 
+// Plain rec-side path (k_eval): catalog rows per tile (~16 KB per stage) and its shared-memory limit.
+static int plain_tile_rows(int64_t cat_ld) {
+  int tn = static_cast<int>((16 * 1024) / (cat_ld * sizeof(float)));
+  tn = tn < 4 ? 4 : (tn > 64 ? 64 : tn);
+  return tn & ~3;
+}
+constexpr int kPlainSmemLimit = 220 * 1024;
+
 static int eval_rotate() {
   static const int v = [] { const char* e = getenv("KGREC_EVAL_ROTATE"); return (e && e[0] == '0') ? 0 : 1; }();
   return v;
@@ -1453,15 +1461,20 @@ static int eval_plan(const kgrec_tables* T, int model, int side, int mode, const
   if (pl->tiled) {
     // register tile 8 x RN per thread, W warps per CTA.  d <= 128: 16 warps, DIST 8x4 / HYPER 8x2
     // (HYPER keeps two tiles: dots and distances); wider rows: 8 warps, 8x2 / 8x1 to fit smem.
-    const bool wide = d > 128;
-    pl->warps = wide ? 8 : 16;
-    pl->rn = (pl->kind == KIND_DIST ? 4 : 2) / (wide ? 2 : 1);
-    const int tn_t = 32 * pl->rn;
-    int stages = 4;
-    while (stages > 2 && tiled_smem_layout(pl->kind, mode, d, tn_t, stages, k, pl->warps, 0, excl).total > 210 * 1024) --stages;
-    pl->stages = stages;
+    // When the layout does not fit (long top-K lists: TQT * k keys), fall back to 8 warps, then (top-K only) to
+    // 4 warps with the same register tile: fewer queries per CTA, so shorter list and query tiles.
+    int tn_t = 0;
+    for (int warps = d > 128 ? 8 : 16;; warps /= 2) {
+      pl->warps = warps;
+      pl->rn = (pl->kind == KIND_DIST ? 4 : 2) / (warps == 16 ? 1 : 2);
+      tn_t = 32 * pl->rn;
+      int stages = 4;
+      while (stages > 2 && tiled_smem_layout(pl->kind, mode, d, tn_t, stages, k, warps, 0, excl).total > 210 * 1024) --stages;
+      pl->stages = stages;
+      pl->smem = tiled_smem_layout(pl->kind, mode, d, tn_t, stages, k, warps, 0, excl).total;
+      if (pl->smem <= 225 * 1024 || warps == 4 || (warps == 8 && mode != MODE_TOPK)) break;
+    }
     pl->tn = tn_t;
-    pl->smem = tiled_smem_layout(pl->kind, mode, d, tn_t, stages, k, pl->warps, 0, excl).total;
     if (pl->smem > 225 * 1024) { set_error("eval: shared-memory budget exceeded (%zu bytes)", pl->smem); return KGREC_ERR_UNSUPPORTED; }
     const int64_t n_tiles_t = (n_cat + tn_t - 1) / tn_t;
     const int tqt = RQ * pl->warps;
@@ -1477,10 +1490,7 @@ static int eval_plan(const kgrec_tables* T, int model, int side, int mode, const
     A->n_splits = pl->n_splits; A->tn = tn_t; A->k = k;
     return KGREC_OK;
   }
-  // tile rows: ~16 KB per stage
-  int tn = static_cast<int>((16 * 1024) / (cat_ld * sizeof(float)));
-  tn = tn < 4 ? 4 : (tn > 64 ? 64 : tn);
-  tn &= ~3;
+  const int tn = plain_tile_rows(cat_ld);
   pl->tn = tn;
   const int64_t n_tiles = (n_cat + tn - 1) / tn;
   // catalog ranges per query tile: fill the resident CTA slots (3 per SM) without a second wave
@@ -1489,7 +1499,12 @@ static int eval_plan(const kgrec_tables* T, int model, int side, int mode, const
   if (splits > 65535) splits = 65535;
   pl->n_splits = static_cast<int>(splits);
   pl->smem = eval_smem_layout(pl->kind, mode, d, cat_ld, T->n_pref, tn, k).total;
-  if (pl->smem > 220 * 1024) { set_error("eval: shared-memory budget exceeded (%zu bytes)", pl->smem); return KGREC_ERR_UNSUPPORTED; }
+  if (pl->smem > kPlainSmemLimit) {
+    // the preference tables are staged whole (2 x preference_total x embedding_size floats) next to the top-K lists
+    set_error("eval: the rec-side kernel needs %zu bytes of shared memory at embedding_size %d, preference_total %d, topn %d: "
+              "over its %d-byte limit (kgrec_pref_eval_supported states the limit)", pl->smem, d, T->n_pref, k, kPlainSmemLimit);
+    return KGREC_ERR_UNSUPPORTED;
+  }
   A->T = *T; A->rotate = eval_rotate();
   A->side = side;
   A->nq = nq;
@@ -1530,12 +1545,20 @@ static int launch_eval(const EvalArgs& A, const EvalPlan& pl, cudaStream_t st, c
     KGREC_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(pl.smem))); \
     kern<<<pl.grid, WV * 32, pl.smem, st>>>(A, pl.stages, pl.units_per_cta, X);                               \
   }
-    if (pl.kind == KIND_DIST) { if (pl.warps == 16) KGREC_TILED_CASE(KIND_DIST, 4, 16) else KGREC_TILED_CASE(KIND_DIST, 2, 8) }
+    if (pl.kind == KIND_DIST) {
+      if (pl.warps == 16) KGREC_TILED_CASE(KIND_DIST, 4, 16)
+      else if (pl.warps == 8) KGREC_TILED_CASE(KIND_DIST, 2, 8)
+      else if constexpr (MODE == MODE_TOPK) KGREC_TILED_CASE(KIND_DIST, 2, 4)      // eval_plan: 4 warps for top-K only
+    }
     else if (pl.kind == KIND_GUMBEL_L2) {
       if constexpr (MODE == MODE_RANK) { set_error("rank counts are built for the KG sides"); return KGREC_ERR_UNSUPPORTED; }
       else { if (pl.warps == 16) KGREC_TILED_CASE(KIND_GUMBEL_L2, 2, 16) else KGREC_TILED_CASE(KIND_GUMBEL_L2, 1, 8) }
     }
-    else { if (pl.warps == 16) KGREC_TILED_CASE(KIND_HYPER, 2, 16) else KGREC_TILED_CASE(KIND_HYPER, 1, 8) }
+    else {
+      if (pl.warps == 16) KGREC_TILED_CASE(KIND_HYPER, 2, 16)
+      else if (pl.warps == 8) KGREC_TILED_CASE(KIND_HYPER, 1, 8)
+      else if constexpr (MODE == MODE_TOPK) KGREC_TILED_CASE(KIND_HYPER, 1, 4)
+    }
 #undef KGREC_TILED_CASE
     KGREC_CUDA_OK(cudaGetLastError());
     return KGREC_OK;
@@ -1788,6 +1811,17 @@ extern "C" int kgrec_gumbel_aug_rows(const kgrec_tables* tables, int model, cons
 }
 
 extern "C" int32_t kgrec_pref_aug_ld(int32_t dim) { return pref_aug_ld(dim); }
+
+extern "C" int32_t kgrec_pref_aug_supported(int32_t dim, int32_t k) {
+  if (dim <= 0 || dim > 256 || dim % 4 || k < 0 || k > 128) return 0;
+  return soft_smem_layout(k > 0 ? MODE_TOPK : MODE_FULL, pref_aug_ld(dim), 2, k, 8).total <= 225 * 1024;
+}
+
+extern "C" int32_t kgrec_pref_eval_supported(int32_t dim, int32_t n_pref, int32_t use_gumbel, int32_t k) {
+  if (dim <= 0 || dim > 256 || dim % 4 || n_pref <= 0 || n_pref > kMaxPref || k < 0 || k > 128) return 0;
+  return eval_smem_layout(use_gumbel ? KIND_PREF_HARD : KIND_PREF_SOFT, k > 0 ? MODE_TOPK : MODE_FULL, dim, dim, n_pref,
+                          plain_tile_rows(dim), k).total <= kPlainSmemLimit;
+}
 
 extern "C" int kgrec_pref_aug_rows(const kgrec_tables* tables, int model, int is_query, const void* ids, int idx_bytes,
                                    const float* rows, int64_t row_ld, int64_t n, float* out, int64_t ld_out,

@@ -185,6 +185,8 @@ _SIGNATURES = {
     "kgrec_gumbel_aug_rows": (C.c_int, [C.POINTER(Tables), C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_int64, C.c_int64,
                                         C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]),
     "kgrec_pref_aug_ld": (C.c_int32, [C.c_int32]),
+    "kgrec_pref_aug_supported": (C.c_int32, [C.c_int32, C.c_int32]),
+    "kgrec_pref_eval_supported": (C.c_int32, [C.c_int32, C.c_int32, C.c_int32, C.c_int32]),
     "kgrec_pref_aug_rows": (C.c_int, [C.POINTER(Tables), C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_int64,
                                       C.c_int64, C.c_void_p, C.c_int64, C.c_void_p]),
     "kgrec_ktup_item_table": (C.c_int, [C.POINTER(Tables), C.c_int64, C.c_int64, C.c_void_p, C.c_int64,

@@ -381,7 +381,7 @@ class RecEvaluator:
             cat = m.gumbel_catalog()
             qrows = m._gumbel_rows(user_rows, ids=self.users, with_consts=True)
             return m._eval(m.MODEL, _lib.SIDE_REC, None, None, "topk", catalog=cat, qvec=qrows, gumbel_u=gumbel_u, seed=seed, **kw)
-        if not m.use_st_gumbel and m.embedding_size % 4 == 0 and m.embedding_size <= 256:
+        if m._pref_aug_ok(k):
             cat = m.soft_catalog()
             qrows = m._aug_rows(user_rows, True, ids=self.users)
             return m._eval(m.MODEL, _lib.SIDE_REC, None, None, "topk", catalog=cat, qvec=qrows, **kw)

@@ -137,16 +137,24 @@ class KGRecModule(nn.Module):
     def _finish_init(self):
         """The reference moves every table to the GPU when one is visible (misc.py:11-16)."""
         d = self.embedding_size
+        import warnings
         if d % 4 or d > self.EVAL_MAX_DIM:
             # the reference's drivers call evaluate* eval_interval_steps into a run: say so now, not there
-            import warnings
             warnings.warn("kgrec_b200: %s with embedding_size %d can be trained but not evaluated: evaluate* / topk need a "
                           "multiple of 4, <= %d (the call will raise)" % (type(self).__name__, d, self.EVAL_MAX_DIM),
                           stacklevel=3)
+        else:
+            msg = self._eval_envelope_warning()
+            if msg:
+                warnings.warn("kgrec_b200: " + msg, stacklevel=3)
         self._check_every = int(os.environ.get("KGREC_CHECK_EVERY", "0"))
         self._calls = 0
         if torch.cuda.is_available():
             self.cuda()
+
+    def _eval_envelope_warning(self):
+        """A shape-dependent limit of the evaluation kernels inside the embedding_size rule, or None."""
+        return None
 
     def _maybe_check(self):
         """Out-of-range ids: the kernels clamp them to row 0 and raise a device status word (the reference's

@@ -71,9 +71,37 @@ class RecModelBase(KGRecModule):
             return False
         return bool(_lib.load().kgrec_gumbel_aug_supported(self.embedding_size, self.pref_embeddings.weight.shape[0], k))
 
+    def _pref_aug_ok(self, k=0):
+        """Soft preferences on augmented rows (k_eval_soft); False -> the plain path on user / item ids."""
+        if self.use_st_gumbel:
+            return False
+        return bool(_lib.load().kgrec_pref_aug_supported(self.embedding_size, k))
+
+    def rec_eval_max_topn(self):
+        """Largest topn (<= 128) that topk_items / RecEvaluator serve at this model's shape: 0 when only the score
+        matrix (evaluate / evaluateRec) can be computed, -1 when not even that."""
+        d, P = self.embedding_size, self.pref_embeddings.weight.shape[0]
+        if d % 4 or d > self.EVAL_MAX_DIM:
+            return -1
+        lib = _lib.load()
+
+        def ok(k):
+            return self._gumbel_aug_ok(k) or self._pref_aug_ok(k) or bool(lib.kgrec_pref_eval_supported(d, P, int(self.use_st_gumbel), k))
+        return max([k for k in range(0, 129) if ok(k)] or [-1])
+
+    def _eval_envelope_warning(self):
+        k = self.rec_eval_max_topn()
+        if k < 128:
+            what = "evaluate / evaluateRec / topk_items raise" if k < 0 else "topk_items / RecEvaluator need topn <= %d" % k
+            return ("%s with embedding_size %d and preference_total %d: %s (the rec-side kernel stages both preference "
+                    "tables in shared memory; see kgrec_pref_eval_supported)"
+                    % (type(self).__name__, self.embedding_size, self.pref_embeddings.weight.shape[0], what))
+        return None
+
     def _rec_call(self, mode, u_ids, gumbel_u, catalog, soft_catalog, **kw):
         dev = self._require_cuda()
-        if self._gumbel_aug_ok(kw.get("k", 10) if mode == "topk" else 0):
+        k = kw.get("k", 10) if mode == "topk" else 0
+        if self._gumbel_aug_ok(k):
             # ST-Gumbel, squared L2: the tiled distance kernel on augmented rows + a per-pair arg-max epilogue
             u = KF.as_index(u_ids, dev)
             if u.numel() == 0:
@@ -83,8 +111,7 @@ class RecModelBase(KGRecModule):
             seed = self._next_seed() if gumbel_u is None else 0
             return self._eval(self.MODEL, _lib.SIDE_REC, None, None, mode, catalog=aug_cat, qvec=qrows, gumbel_u=gumbel_u,
                               seed=seed, **kw)
-        use_aug = (not self.use_st_gumbel) and self.embedding_size % 4 == 0 and self.embedding_size <= 256
-        if use_aug:
+        if self._pref_aug_ok(k):
             u = KF.as_index(u_ids, dev)
             if u.numel() == 0:
                 return self._eval(self.MODEL, _lib.SIDE_REC, u, None, mode, catalog=self._rec_catalog(), **kw)
