@@ -514,14 +514,50 @@ int kgrec_eval_rank_count(const kgrec_tables* tables, int model, int side,
  * where X_i = excl_ids[excl_ptr[excl_row[i]], excl_ptr[excl_row[i] + 1]) holds ascending GLOBAL ids
  * (the query's filter set -- train + other eval files -- and its gold set; the gold itself never
  * counts, the comparison being strict).  Rows that share a query share its exclusion row.  An id is
- * looked up only when its key is below the gold's.  Shard counts still add.  KG sides only; all
- * three arrays are required (an empty exclusion is a CSR of empty rows). */
+ * looked up only when its key is below the gold's.  Shard counts still add.  KG sides only (the rec side:
+ * kgrec_rec_rank_count); all three arrays are required (an empty exclusion is a CSR of empty rows). */
 int kgrec_eval_rank_count_ex(const kgrec_tables* tables, int model, int side,
                              const void* q, const void* r, int idx_bytes, const float* qvec, int64_t nq,
                              const float* cat, int64_t cat_ld, int64_t n_cat, int64_t id_base,
                              const float* gold_scores, const int32_t* gold_ids, int32_t* counts,
                              const int32_t* excl_row, const int64_t* excl_ptr, const int32_t* excl_ids,
                              kgrec_stream_t stream);
+
+/* Rank counts of the recommendation side (TUP / KTUP): where every gold item of a user sits in the whole filtered
+ * catalog.  The queries are USERS, one query per user exactly as in kgrec_eval_topk on KGREC_SIDE_REC (q = user ids,
+ * or qvec = augmented user rows with cat = the augmented catalog of the same kind: kgrec_pref_aug_rows /
+ * kgrec_gumbel_aug_rows; the three paths and their envelopes are those of kgrec_eval_scores).  The hashed ST-Gumbel
+ * noise is one draw per (position of the user in the call, global item id, preference), so only a call with the same
+ * user list and seed ranks by the scores kgrec_eval_topk / kgrec_eval_scores see.  The golds hang off the query as a
+ * CSR: G_q = gold_ids[gold_ptr[q], gold_ptr[q + 1]) (ascending global ids, n_gold = gold_ptr[nq] in all); the filter
+ * row F_q = filter_ids[filter_ptr[q], filter_ptr[q + 1]) is the CSR kgrec_eval_topk takes (both NULL: no filter).
+ *
+ *   counts[j] += #{ e in shard : (score(u_q, e), e) < (score(u_q, g_j), g_j), e not in F_q, e not in G_q }
+ *                                                                            gold_ptr[q] <= j < gold_ptr[q + 1]
+ *
+ * in the (score bits, global id) key order of kgrec_eval_topk, strictly: a gold never counts itself and two golds of
+ * one user never count each other.  This is getKGPerformance's rank (utils/misc.py:125-146) in getRecPerformance's
+ * order and filter (213-229).  A gold that is itself in F_q (never in the top-n list either) is skipped: the call
+ * SETS its count to -1.  Counts (caller-zeroed) of different catalog shards add, so after the sum a skipped gold is
+ * negative.
+ *
+ * The gold scores must be the values the count pass computes itself, bit for bit, noise included.
+ * kgrec_rec_gold_scores is therefore a sweep of the same kernels over the shard that stores the score of every
+ * (q, g_j) pair it meets: gold_scores[j] (caller-zeroed) is written when g_j lies in the shard, so the arrays of
+ * different shards add (scores are >= 0 and every gold lives in one shard).  kgrec_rec_rank_count then sorts each
+ * query's gold keys, streams the shard once more and, for every pair below the query's largest gold key, finds by
+ * binary search the golds it sorts before; the filter row is searched only for such pairs.  Any number of golds per
+ * query.  workspace: kgrec_rec_rank_workspace_bytes(nq, n_gold) bytes, 8-byte aligned.  nq = 0 or n_gold = 0: no-op. */
+int kgrec_rec_gold_scores(const kgrec_tables* tables, int model, const void* q, int idx_bytes, const float* qvec,
+                          int64_t nq, const float* cat, int64_t cat_ld, int64_t n_cat, int64_t id_base,
+                          const int64_t* gold_ptr, const int32_t* gold_ids, const float* gumbel_u, uint64_t seed,
+                          float* gold_scores, kgrec_stream_t stream);
+int64_t kgrec_rec_rank_workspace_bytes(int64_t nq, int64_t n_gold);
+int kgrec_rec_rank_count(const kgrec_tables* tables, int model, const void* q, int idx_bytes, const float* qvec,
+                         int64_t nq, const float* cat, int64_t cat_ld, int64_t n_cat, int64_t id_base,
+                         const int64_t* gold_ptr, const int32_t* gold_ids, int64_t n_gold, const float* gold_scores,
+                         const int64_t* filter_ptr, const int32_t* filter_ids, const float* gumbel_u, uint64_t seed,
+                         int32_t* counts, void* workspace, int64_t workspace_bytes, kgrec_stream_t stream);
 
 /* Per-user top-n metrics of the rec side (getRecPerformance, utils/misc.py:213-248): keys [nq, k] from
  * kgrec_eval_topk (UINT64_MAX places are not part of the list), gold sets as a CSR (gold_ptr [nq+1],

@@ -25,7 +25,7 @@
 namespace kgrec {
 
 enum { KIND_DIST = 0, KIND_HYPER = 1, KIND_PREF_HARD = 2, KIND_PREF_SOFT = 3, KIND_GUMBEL_L2 = 4 };
-enum { MODE_FULL = 0, MODE_TOPK = 1, MODE_RANK = 2 };
+enum { MODE_FULL = 0, MODE_TOPK = 1, MODE_RANK = 2, MODE_RRANK = 3 };   // RRANK: rank counts of the rec side, golds as a CSR per query
 
 constexpr int QW = 8;                       // queries per warp
 constexpr int TQ = QW * kWarpsPerCta;       // queries per CTA
@@ -107,7 +107,55 @@ struct EvalArgs {
   uint32_t* thr_glob;                       // TOPK, tiled kernels: [nq] score bits no top-K entry of the call can exceed (shared by the pieces)
   const int64_t* filter_ptr; const int32_t* filter_ids;
   const float* gold_scores; const int32_t* gold_ids; int32_t* counts;   // RANK
+  // RRANK (gold_ids is the CSR's id array): query q owns the golds [gold_ptr[q], gold_ptr[q + 1])
+  const int64_t* gold_ptr;
+  float* gold_out;              // capture pass (gold_keys == NULL): [n_gold] scores of the golds met in this shard
+  const uint64_t* gold_keys;    // count pass: every query's gold keys in ascending order
+  const int32_t* gold_perm;     //   CSR position of the sorted gold, ~position when the gold is filtered (its key is 0)
+  const uint64_t* gold_max;     //   [nq] largest gold key of the query
+  int32_t* gold_diff;           //   [n_gold] difference array of the counts in sorted order
 };
+
+// MODE_RRANK: what the three rec-side kernels do with one scored (query, item) pair; called by whole warps.
+//   capture pass: an item that is one of the query's golds stores its score, so the count pass compares the golds
+//     with values of its own arithmetic and noise.
+//   count pass: a pair below the query's largest gold key finds by binary search the first sorted gold it sorts
+//     before (position p); unless it is a gold itself or in the query's filter row, every gold from p on counts
+//     it: +1 at p of the difference array, whose prefix sums are the counts (k_rec_rank_finish).  Lanes that hit
+//     the same position share one atomic.
+__device__ __forceinline__ void rrank_pair(const EvalArgs& A, bool valid, int64_t q, uint32_t sb, uint32_t id, uint64_t gmax, int lane) {
+  if (!A.gold_keys) {
+    if (valid) {
+      int64_t lo = __ldg(A.gold_ptr + q), hi = __ldg(A.gold_ptr + q + 1);
+      while (lo < hi) {
+        const int64_t mid = (lo + hi) >> 1;
+        const int32_t v = __ldg(A.gold_ids + mid);
+        if (v == static_cast<int32_t>(id)) { A.gold_out[mid] = __uint_as_float(sb); break; }
+        if (v < static_cast<int32_t>(id)) lo = mid + 1; else hi = mid;
+      }
+    }
+    return;
+  }
+  const uint64_t key = (static_cast<uint64_t>(sb) << 32) | id;
+  int64_t p = -1;
+  if (valid && key < gmax) {
+    int64_t lo = __ldg(A.gold_ptr + q), hi = __ldg(A.gold_ptr + q + 1);
+    while (lo < hi) {                       // ends below the row's end: key < gmax
+      const int64_t mid = (lo + hi) >> 1;
+      if (__ldg(A.gold_keys + mid) < key) lo = mid + 1; else hi = mid;
+    }
+    const bool is_gold = __ldg(A.gold_keys + lo) == key && __ldg(A.gold_perm + lo) >= 0;
+    if (!is_gold && !(A.filter_ptr && filtered(A.filter_ids, __ldg(A.filter_ptr + q), __ldg(A.filter_ptr + q + 1), static_cast<int32_t>(id))))
+      p = lo;
+  }
+  unsigned todo = __ballot_sync(FULL, p >= 0);
+  while (todo) {                            // warp-uniform: one round per distinct position among the lanes
+    const int src = __ffs(todo) - 1;
+    const unsigned same = __ballot_sync(FULL, p == __shfl_sync(FULL, p, src));
+    if (lane == src) atomicAdd(A.gold_diff + p, __popc(same));
+    todo &= ~same;
+  }
+}
 
 // smem carve-up (floats unless noted), in this order:
 //   bars        : 2 * kStages uint64
@@ -304,6 +352,9 @@ k_eval(const EvalArgs A) {
   if constexpr (MODE == MODE_RANK) {
     if (q_valid) gold_key = make_key(__ldg(A.gold_scores + my_query), static_cast<uint32_t>(__ldg(A.gold_ids + my_query)));
   }
+  if constexpr (MODE == MODE_RRANK) {
+    if (q_valid && A.gold_max) gold_key = __ldg(A.gold_max + my_query);
+  }
 
   for (int64_t t = 0; t < my_tiles; ++t) {
     const int s = static_cast<int>(t % kStages);
@@ -470,6 +521,8 @@ k_eval(const EvalArgs A) {
         if (valid) A.out[my_query * A.ld_out + n_local] = mine;
       } else if constexpr (MODE == MODE_RANK) {
         if (valid && make_key(mine, static_cast<uint32_t>(A.id_base + n_local)) < gold_key) ++cnt;
+      } else if constexpr (MODE == MODE_RRANK) {
+        rrank_pair(A, valid, my_query, __float_as_uint(mine), static_cast<uint32_t>(A.id_base + n_local), gold_key, lane);
       } else {
         const uint64_t key = make_key(mine, static_cast<uint32_t>(A.id_base + n_local));
         bool pass = valid && key < thr;
@@ -958,6 +1011,8 @@ k_eval_tiled(const EvalArgs A, const int stages, const int64_t units_per_cta, co
           } else {
             if (valid && (sb < gh || (sb == gh && id < gi))) ++cnt[qi];
           }
+        } else if constexpr (MODE == MODE_RRANK) {
+          rrank_pair(A, valid, q, sb, static_cast<uint32_t>(A.id_base + n_local), A.gold_max ? __ldg(A.gold_max + q) : 0ull, lane);
         } else {
           const unsigned mask = __ballot_sync(FULL, valid && sb <= thr_hi[qi]);
           if (mask) {                            // rare once the lists have warmed up
@@ -1231,6 +1286,8 @@ k_eval_soft(const EvalArgs A, const int stages, const int64_t units_per_cta) {
       const float sc = sum2(acc2[qi]);
       if constexpr (MODE == MODE_FULL) {
         if (valid) __stcs(A.out + q * A.ld_out + n_local, sc);
+      } else if constexpr (MODE == MODE_RRANK) {
+        rrank_pair(A, valid, q, __float_as_uint(sc), static_cast<uint32_t>(A.id_base + n_local), A.gold_max ? __ldg(A.gold_max + q) : 0ull, lane);
       } else {
         const uint32_t sb = __float_as_uint(sc);
         const unsigned mask = __ballot_sync(FULL, valid && sb <= thr_hi[qi]);
@@ -1580,6 +1637,118 @@ static int launch_eval(const EvalArgs& A, const EvalPlan& pl, cudaStream_t st, c
   return KGREC_OK;
 }
 
+// Count pass of the rec-side rank mode, step 1: one warp per query turns its golds (CSR order, ascending ids) into keys
+// sorted ascending.  A gold that is in the query's filter row is skipped by the definition: its key is 0, which no pair
+// sorts before, and its perm entry is ~position.  tmp holds the unsorted keys; golds per query are few, so the order is
+// found by counting smaller keys.
+__global__ void __launch_bounds__(256)
+k_rec_gold_prep(int64_t nq, const int64_t* __restrict__ gold_ptr, const int32_t* __restrict__ gold_ids,
+                const float* __restrict__ gold_scores, const int64_t* __restrict__ filter_ptr,
+                const int32_t* __restrict__ filter_ids, uint64_t* tmp, uint64_t* __restrict__ keys,
+                int32_t* __restrict__ perm, uint64_t* __restrict__ gmax) {
+  const int lane = threadIdx.x & 31;
+  for (int64_t q = static_cast<int64_t>(blockIdx.x) * 8 + (threadIdx.x >> 5); q < nq; q += static_cast<int64_t>(gridDim.x) * 8) {
+    const int64_t lo = __ldg(gold_ptr + q), hi = __ldg(gold_ptr + q + 1);
+    const int64_t f_lo = filter_ptr ? __ldg(filter_ptr + q) : 0, f_hi = filter_ptr ? __ldg(filter_ptr + q + 1) : 0;
+    uint64_t mx = 0;
+    for (int64_t j = lo + lane; j < hi; j += 32) {
+      const int32_t id = __ldg(gold_ids + j);
+      const uint64_t key = filtered(filter_ids, f_lo, f_hi, id) ? 0ull : make_key(__ldg(gold_scores + j), static_cast<uint32_t>(id));
+      tmp[j] = key;
+      mx = key > mx ? key : mx;
+    }
+    __syncwarp();
+    for (int64_t j = lo + lane; j < hi; j += 32) {
+      const uint64_t key = tmp[j];
+      int64_t rank = 0;
+      for (int64_t i = lo; i < hi; ++i) {
+        const uint64_t other = tmp[i];
+        rank += (other < key || (other == key && i < j)) ? 1 : 0;
+      }
+      keys[lo + rank] = key;
+      perm[lo + rank] = static_cast<int32_t>(filtered(filter_ids, f_lo, f_hi, __ldg(gold_ids + j)) ? ~j : j);
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) { const uint64_t v = __shfl_xor_sync(FULL, mx, o); mx = v > mx ? v : mx; }
+    if (lane == 0) gmax[q] = mx;
+  }
+}
+
+// Step 3: the counts are the prefix sums of the difference array in sorted order; a filtered gold reads -1.
+__global__ void __launch_bounds__(256)
+k_rec_rank_finish(int64_t nq, const int64_t* __restrict__ gold_ptr, const int32_t* __restrict__ perm,
+                  const int32_t* __restrict__ diff, int32_t* __restrict__ counts) {
+  const int lane = threadIdx.x & 31;
+  for (int64_t q = static_cast<int64_t>(blockIdx.x) * 8 + (threadIdx.x >> 5); q < nq; q += static_cast<int64_t>(gridDim.x) * 8) {
+    const int64_t lo = __ldg(gold_ptr + q), hi = __ldg(gold_ptr + q + 1);
+    int carry = 0;
+    for (int64_t base = lo; base < hi; base += 32) {
+      const int64_t j = base + lane;
+      int v = j < hi ? __ldg(diff + j) : 0;
+#pragma unroll
+      for (int o = 1; o < 32; o <<= 1) { const int t = __shfl_up_sync(FULL, v, o); if (lane >= o) v += t; }
+      if (j < hi) {
+        const int32_t pj = __ldg(perm + j);
+        if (pj >= 0) counts[pj] += carry + v; else counts[~pj] = -1;
+      }
+      carry += __shfl_sync(FULL, v, 31);
+    }
+  }
+}
+
+// the three rec-side kernels in the rank mode (capture or count pass: A.gold_keys)
+static int launch_rec_rank(const EvalArgs& A, const EvalPlan& pl, cudaStream_t st) {
+#define KGREC_RRANK_LAUNCH(KERN, GRID, THREADS, ...)                                                          \
+  {                                                                                                           \
+    auto kern = KERN;                                                                                         \
+    KGREC_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(pl.smem))); \
+    kern<<<GRID, THREADS, pl.smem, st>>>(__VA_ARGS__);                                                        \
+  }
+  const dim3 grid(static_cast<unsigned>(pl.n_qtiles), static_cast<unsigned>(pl.n_splits));
+  if (pl.soft_aug) {
+    if (A.T.l1) KGREC_RRANK_LAUNCH((k_eval_soft<MODE_RRANK, true, 8>), pl.grid, 8 * 32, A, pl.stages, pl.units_per_cta)
+    else KGREC_RRANK_LAUNCH((k_eval_soft<MODE_RRANK, false, 8>), pl.grid, 8 * 32, A, pl.stages, pl.units_per_cta)
+  } else if (pl.tiled) {
+    if (pl.warps == 16) KGREC_RRANK_LAUNCH((k_eval_tiled<KIND_GUMBEL_L2, MODE_RRANK, false, 2, 16, false>), pl.grid, 16 * 32, A, pl.stages, pl.units_per_cta, ExclArgs{})
+    else KGREC_RRANK_LAUNCH((k_eval_tiled<KIND_GUMBEL_L2, MODE_RRANK, false, 1, 8, false>), pl.grid, 8 * 32, A, pl.stages, pl.units_per_cta, ExclArgs{})
+  } else if (pl.kind == KIND_PREF_HARD) {
+    if (pl.nch == 1) { if (A.T.l1) KGREC_RRANK_LAUNCH((k_eval<KIND_PREF_HARD, 1, MODE_RRANK, true>), grid, kEvalThreads, A) else KGREC_RRANK_LAUNCH((k_eval<KIND_PREF_HARD, 1, MODE_RRANK, false>), grid, kEvalThreads, A) }
+    else { if (A.T.l1) KGREC_RRANK_LAUNCH((k_eval<KIND_PREF_HARD, 2, MODE_RRANK, true>), grid, kEvalThreads, A) else KGREC_RRANK_LAUNCH((k_eval<KIND_PREF_HARD, 2, MODE_RRANK, false>), grid, kEvalThreads, A) }
+  } else {
+    if (pl.nch == 1) { if (A.T.l1) KGREC_RRANK_LAUNCH((k_eval<KIND_PREF_SOFT, 1, MODE_RRANK, true>), grid, kEvalThreads, A) else KGREC_RRANK_LAUNCH((k_eval<KIND_PREF_SOFT, 1, MODE_RRANK, false>), grid, kEvalThreads, A) }
+    else { if (A.T.l1) KGREC_RRANK_LAUNCH((k_eval<KIND_PREF_SOFT, 2, MODE_RRANK, true>), grid, kEvalThreads, A) else KGREC_RRANK_LAUNCH((k_eval<KIND_PREF_SOFT, 2, MODE_RRANK, false>), grid, kEvalThreads, A) }
+  }
+#undef KGREC_RRANK_LAUNCH
+  KGREC_CUDA_OK(cudaGetLastError());
+  return KGREC_OK;
+}
+
+// argument checks and launch plan shared by kgrec_rec_gold_scores and kgrec_rec_rank_count; *empty: nothing to launch
+static int rec_rank_plan(const char* who, const kgrec_tables* tables, int model, const void* q, int idx_bytes, const float* qvec,
+                         int64_t nq, const float* cat, int64_t cat_ld, int64_t n_cat, int64_t id_base, const int64_t* gold_ptr,
+                         const int32_t* gold_ids, const float* gumbel_u, uint64_t seed, EvalArgs* A, EvalPlan* pl, bool* empty) {
+  *empty = false;
+  if (model != KGREC_TUP && model != KGREC_KTUP) { set_error("%s: model %d is not a recommendation model (TUP / KTUP)", who, model); return KGREC_ERR_INVALID; }
+  if (nq < 0) { set_error("%s: nq must be >= 0", who); return KGREC_ERR_INVALID; }
+  if (nq == 0) { *empty = true; return KGREC_OK; }
+  const int rc = eval_plan(tables, model, KGREC_SIDE_REC, MODE_RRANK, cat, cat_ld, nq, n_cat, 0, qvec != nullptr, A, pl);
+  if (rc) return rc;
+  if (!gold_ptr || !gold_ids) { set_error("%s: NULL argument (gold_ptr / gold_ids)", who); return KGREC_ERR_INVALID; }
+  if ((reinterpret_cast<uintptr_t>(gold_ptr) & 7u) || (reinterpret_cast<uintptr_t>(gold_ids) & 3u)) {
+    set_error("%s: gold CSR arrays are not aligned to their element size", who);
+    return KGREC_ERR_INVALID;
+  }
+  if (!qvec && !q) { set_error("query ids are NULL"); return KGREC_ERR_INVALID; }
+  if (!qvec && idx_bytes != 4 && idx_bytes != 8) { set_error("idx_bytes must be 4 or 8"); return KGREC_ERR_INVALID; }
+  if (id_base < 0 || id_base + n_cat > 0x7fffffffll) { set_error("catalog ids must fit 32 bits (gold and filter ids are int32)"); return KGREC_ERR_INVALID; }
+  A->q = q; A->is64 = idx_bytes == 8; A->qvec = qvec;
+  A->qvec_ld = pl->kind == KIND_GUMBEL_L2 ? cat_ld : 2 * static_cast<int64_t>(tables->dim);
+  A->gconst = pl->kind == KIND_GUMBEL_L2 ? qvec + nq * cat_ld : nullptr;     // the constants follow the query rows
+  A->gumbel_u = gumbel_u; A->seed = seed; A->id_base = id_base;
+  A->gold_ptr = gold_ptr; A->gold_ids = gold_ids;
+  return KGREC_OK;
+}
+
 }  // namespace kgrec
 
 using namespace kgrec;
@@ -1707,6 +1876,69 @@ extern "C" int kgrec_eval_rank_count_ex(const kgrec_tables* tables, int model, i
   const ExclArgs X{excl_row, excl_ptr, excl_ids};
   return rank_count(tables, model, side, q, r, idx_bytes, qvec, nq, cat, cat_ld, n_cat, id_base, gold_scores, gold_ids, counts,
                     &X, stream);
+}
+
+extern "C" int kgrec_rec_gold_scores(const kgrec_tables* tables, int model, const void* q, int idx_bytes, const float* qvec,
+                                     int64_t nq, const float* cat, int64_t cat_ld, int64_t n_cat, int64_t id_base,
+                                     const int64_t* gold_ptr, const int32_t* gold_ids, const float* gumbel_u, uint64_t seed,
+                                     float* gold_scores, kgrec_stream_t stream) {
+  EvalArgs A{};
+  EvalPlan pl{};
+  bool empty;
+  const int rc = rec_rank_plan("rec_gold_scores", tables, model, q, idx_bytes, qvec, nq, cat, cat_ld, n_cat, id_base, gold_ptr,
+                               gold_ids, gumbel_u, seed, &A, &pl, &empty);
+  if (rc || empty) return rc;
+  if (!gold_scores) { set_error("rec_gold_scores: NULL argument (gold_scores)"); return KGREC_ERR_INVALID; }
+  A.gold_out = gold_scores;
+  return launch_rec_rank(A, pl, static_cast<cudaStream_t>(stream));
+}
+
+extern "C" int64_t kgrec_rec_rank_workspace_bytes(int64_t nq, int64_t n_gold) {
+  return 8 * (nq > 0 ? nq : 0) + 24 * (n_gold > 0 ? n_gold : 0) + 16;
+}
+
+extern "C" int kgrec_rec_rank_count(const kgrec_tables* tables, int model, const void* q, int idx_bytes, const float* qvec,
+                                    int64_t nq, const float* cat, int64_t cat_ld, int64_t n_cat, int64_t id_base,
+                                    const int64_t* gold_ptr, const int32_t* gold_ids, int64_t n_gold, const float* gold_scores,
+                                    const int64_t* filter_ptr, const int32_t* filter_ids, const float* gumbel_u, uint64_t seed,
+                                    int32_t* counts, void* workspace, int64_t workspace_bytes, kgrec_stream_t stream) {
+  EvalArgs A{};
+  EvalPlan pl{};
+  bool empty;
+  int rc = rec_rank_plan("rec_rank_count", tables, model, q, idx_bytes, qvec, nq, cat, cat_ld, n_cat, id_base, gold_ptr, gold_ids,
+                         gumbel_u, seed, &A, &pl, &empty);
+  if (rc || empty) return rc;
+  if (n_gold < 0 || n_gold > 0x7fffffffll) { set_error("rec_rank_count: n_gold out of range"); return KGREC_ERR_INVALID; }
+  if (n_gold == 0) return KGREC_OK;
+  if (!gold_scores || !counts) { set_error("rec_rank_count: NULL argument (gold_scores / counts)"); return KGREC_ERR_INVALID; }
+  if (!filter_ptr != !filter_ids) { set_error("rec_rank_count: filter CSR has one NULL array (pass both, or neither for no filter)"); return KGREC_ERR_INVALID; }
+  if ((reinterpret_cast<uintptr_t>(filter_ptr) & 7u) || (reinterpret_cast<uintptr_t>(filter_ids) & 3u)) {
+    set_error("rec_rank_count: filter CSR arrays are not aligned to their element size");
+    return KGREC_ERR_INVALID;
+  }
+  const int64_t need = kgrec_rec_rank_workspace_bytes(nq, n_gold);
+  if (!workspace || (reinterpret_cast<uintptr_t>(workspace) & 7u) || workspace_bytes < need) {
+    set_error("rec_rank_count: workspace must be 8-byte aligned and hold %lld bytes (kgrec_rec_rank_workspace_bytes)", static_cast<long long>(need));
+    return KGREC_ERR_INVALID;
+  }
+  // workspace: gold_max [nq] | sorted keys [n_gold] | unsorted keys [n_gold] | perm [n_gold] | diff [n_gold]
+  uint64_t* gmax = static_cast<uint64_t*>(workspace);
+  uint64_t* keys = gmax + nq;
+  uint64_t* tmp = keys + n_gold;
+  int32_t* perm = reinterpret_cast<int32_t*>(tmp + n_gold);
+  int32_t* diff = perm + n_gold;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  KGREC_CUDA_OK(cudaMemsetAsync(diff, 0, static_cast<size_t>(n_gold) * sizeof(int32_t), st));
+  const int64_t ctas = (nq + 7) / 8, cap = static_cast<int64_t>(sm_count()) * 16;
+  const unsigned grid = static_cast<unsigned>(ctas < cap ? ctas : cap);
+  k_rec_gold_prep<<<grid, 256, 0, st>>>(nq, gold_ptr, gold_ids, gold_scores, filter_ptr, filter_ids, tmp, keys, perm, gmax);
+  KGREC_CUDA_OK(cudaGetLastError());
+  A.filter_ptr = filter_ptr; A.filter_ids = filter_ids;
+  A.gold_keys = keys; A.gold_perm = perm; A.gold_max = gmax; A.gold_diff = diff;
+  if ((rc = launch_rec_rank(A, pl, st))) return rc;
+  k_rec_rank_finish<<<grid, 256, 0, st>>>(nq, gold_ptr, perm, diff, counts);
+  KGREC_CUDA_OK(cudaGetLastError());
+  return KGREC_OK;
 }
 
 // Per-user top-n metrics of the rec side (getRecPerformance, utils/misc.py:213-248; evaluation.rec_metrics_from_topk):

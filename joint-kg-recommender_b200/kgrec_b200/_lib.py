@@ -165,6 +165,14 @@ _SIGNATURES = {
                                            C.c_void_p]),
     "kgrec_rec_topk_metrics": (C.c_int, [C.c_void_p, C.c_int64, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
                                          C.c_void_p]),
+    "kgrec_rec_gold_scores": (C.c_int, [C.POINTER(Tables), C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_int64, C.c_void_p,
+                                        C.c_int64, C.c_int64, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64,
+                                        C.c_void_p, C.c_void_p]),
+    "kgrec_rec_rank_workspace_bytes": (C.c_int64, [C.c_int64, C.c_int64]),
+    "kgrec_rec_rank_count": (C.c_int, [C.POINTER(Tables), C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_int64, C.c_void_p,
+                                       C.c_int64, C.c_int64, C.c_int64, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p,
+                                       C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_int64,
+                                       C.c_void_p]),
     "kgrec_transr_workspace_floats": (C.c_int64, [C.c_int64, C.c_int64, C.c_int32]),
     "kgrec_transr_eval_scores": (C.c_int, [C.POINTER(Tables), C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_int64,
                                            C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_int64, C.c_int64, C.c_int64,

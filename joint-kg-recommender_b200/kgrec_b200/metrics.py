@@ -355,11 +355,20 @@ class RecEvaluator:
     filtered top-n of every user in one call and reduces them on the device (kgrec_rec_topk_metrics); result(m) reads
     back five numbers.  ST-Gumbel draws come from `seed` (passed by value; one draw per (user position, item,
     preference)) or from explicit uniforms `gumbel_u` [n_users, n_items, P].
+
+    ranks=True adds the whole-catalog numbers of the gold items (RecModelBase.rank_counts_items on the path of the
+    top-n pass, same users, same noise): run() returns ten sums, result(m) (f1, p, r, hit, ndcg, mean_rank, mrr, auc).
+      mean_rank  mean over the kept golds of the filtered 0-based rank (a gold inside its user's filter set is left out)
+      mrr        mean over the kept golds of 1 / (rank + 1)
+      auc        mean over the users with a kept gold and N_u > 0 of 1 - sum(ranks) / (kept golds * N_u), where
+                 N_u = item_total - |filter set U gold set| is the number of unfiltered non-gold items: the share of
+                 (gold, other item) pairs the model orders correctly, which is what the BPR loss optimises
     """
 
-    def __init__(self, model, eval_dict, all_dicts=None, topn=10):
+    def __init__(self, model, eval_dict, all_dicts=None, topn=10, ranks=False):
         self.model = model
         self.topn = int(topn)
+        self.ranks = bool(ranks)
         dev = model._require_cuda()
         users = [u for u, gold in eval_dict.items() if len(gold) > 0]
         a = side_arrays(users, eval_dict, all_dicts, drop_filtered_gold=False)
@@ -371,6 +380,13 @@ class RecEvaluator:
         self.filter_csr = (torch.as_tensor(a["filt_ptr"], device=dev), _dev_ids(a["filt_ids"], dev, torch.int32))
         self.gold_ptr = torch.as_tensor(a["gold_ptr"], device=dev)
         self.gold_ids = _dev_ids(a["gold_ids"], dev, torch.int32)
+        if self.ranks:
+            n_items = model.item_embeddings.weight.shape[0]
+            if a["gold_ids"].size and a["gold_ids"].max() >= n_items:
+                raise IndexError("kgrec_b200: a gold id of the eval dict is out of range for the item table")
+            self.n_gold = int(a["gold_ids"].size)
+            self.gold_user = torch.as_tensor(np.repeat(np.arange(self.n, dtype=np.int64), np.diff(a["gold_ptr"])), device=dev)
+            self.n_other = torch.as_tensor((n_items - np.diff(a["excl_ptr"])).astype(np.float64), device=dev)     # N_u
 
     def topk(self, seed=0, gumbel_u=None):
         """[n_users, topn] filtered top-n keys of the current tables (the dispatch of RecModelBase._rec_call)."""
@@ -403,11 +419,36 @@ class RecEvaluator:
         """[5] float64 device tensor of the per-user sums, queued on the current stream with no host synchronisation
         (the hit sum is an exact count; result() divides on the host, as evaluate_rec's mean does)."""
         if not self.n:
-            return torch.zeros(5, dtype=torch.float64, device=self.model._require_cuda())
-        return self.per_user(seed, gumbel_u).sum(0)
+            return torch.zeros(10 if self.ranks else 5, dtype=torch.float64, device=self.model._require_cuda())
+        five = self.per_user(seed, gumbel_u).sum(0)
+        return torch.cat([five, self.rank_sums(seed, gumbel_u)]) if self.ranks else five
+
+    def rank_counts(self, seed=0, gumbel_u=None):
+        """int32 [n_gold] filtered rank of every gold (gold CSR order; -1: the gold is in its user's filter set)."""
+        m = self.model
+        return m.rank_counts_items(self.users, (self.gold_ptr, self.gold_ids), self.filter_csr, gumbel_u=gumbel_u,
+                                   seed=seed if m.use_st_gumbel else 0, topn=self.topn, n_gold=self.n_gold)
+
+    def rank_sums(self, seed=0, gumbel_u=None):
+        """[5] float64: (rank sum, reciprocal-rank sum, per-user AUC sum, kept golds, users in the AUC mean).  The
+        per-user sums are integer scatter-adds, so the result repeats bit for bit."""
+        c = self.rank_counts(seed, gumbel_u).to(torch.int64)
+        kept = c >= 0
+        c = torch.where(kept, c, torch.zeros_like(c))
+        rr = torch.where(kept, 1.0 / (c.to(torch.float64) + 1.0), torch.zeros((), dtype=torch.float64, device=c.device))
+        s_u = torch.zeros(self.n, dtype=torch.int64, device=c.device).index_add_(0, self.gold_user, c)
+        n_u = torch.zeros(self.n, dtype=torch.int64, device=c.device).index_add_(0, self.gold_user, kept.to(torch.int64))
+        use = (n_u > 0) & (self.n_other > 0)
+        auc = torch.where(use, 1.0 - s_u.to(torch.float64) / (n_u.to(torch.float64) * self.n_other).clamp_min(1.0),
+                          torch.zeros((), dtype=torch.float64, device=c.device))
+        return torch.stack([c.sum().to(torch.float64), rr.sum(), auc.sum(), kept.sum().to(torch.float64),
+                            use.sum().to(torch.float64)])
 
     def result(self, m):
-        """(f1, precision, recall, hit, ndcg) -- evaluate_rec's tuple."""
-        if not self.n:
-            return (0.0,) * 5
-        return tuple(x / self.n for x in m.tolist())
+        """(f1, precision, recall, hit, ndcg) -- evaluate_rec's tuple; with ranks, followed by (mean_rank, mrr, auc)."""
+        v = m.tolist()
+        five = tuple(x / self.n for x in v[:5]) if self.n else (0.0,) * 5
+        if not self.ranks:
+            return five
+        rank_sum, rr_sum, auc_sum, n_kept, n_auc = v[5:]
+        return five + (rank_sum / n_kept if n_kept else 0.0, rr_sum / n_kept if n_kept else 0.0, auc_sum / n_auc if n_auc else 0.0)

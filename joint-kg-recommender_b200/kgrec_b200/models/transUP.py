@@ -133,6 +133,72 @@ class RecModelBase(KGRecModule):
         return self._rec_call("topk", u_ids, gumbel_u, catalog, soft_catalog, id_base=id_base, k=k,
                               filter_csr=filter_csr)
 
+    def _rank_inputs(self, u, catalog, soft_catalog, topn):
+        """(user ids or None, query rows or None, catalog rows) of the path topk_items(k=topn) takes, so that the
+        rank pass scores a pair exactly as that list does."""
+        users = self.user_embeddings.weight.detach()
+        if self._gumbel_aug_ok(topn):
+            cat = soft_catalog if soft_catalog is not None else self.gumbel_catalog(catalog)
+            return None, self._gumbel_rows(users, ids=u, with_consts=True), cat
+        if self._pref_aug_ok(topn):
+            cat = soft_catalog if soft_catalog is not None else self.soft_catalog(catalog)
+            return None, self._aug_rows(users, True, ids=u), cat
+        return u, None, (self._rec_catalog() if catalog is None else catalog).contiguous()
+
+    def _rank_call(self, u_ids, gold_csr, filter_csr, catalog, id_base, soft_catalog, gumbel_u, seed, topn, n_gold, gold_scores):
+        import ctypes as C
+        dev = self._require_cuda()
+        lib = _lib.load()
+        u = KF.as_index(u_ids, dev)
+        gptr, gids = gold_csr
+        n_gold = int(gids.numel()) if n_gold is None else int(n_gold)
+        if gptr.dtype != torch.int64 or gids.dtype != torch.int32 or gptr.numel() != u.numel() + 1:
+            raise ValueError("kgrec_b200: gold_csr is (int64 ptr [n_users + 1], int32 ascending ids)")
+        if u.numel() == 0 or n_gold == 0:
+            return None, n_gold, dev
+        q, qrows, cat = self._rank_inputs(u, catalog, soft_catalog, topn)
+        if gumbel_u is not None:
+            gumbel_u = gumbel_u.to(dev, torch.float32).contiguous()
+        if seed is None:
+            seed = self._next_seed() if (self.use_st_gumbel and gumbel_u is None) else 0
+        T = KF.make_tables(self._weights(), self.embedding_size, self.L1_flag, self.use_st_gumbel, self._item2ent)
+        head = (C.byref(T), self.MODEL, KF._ptr(q), q.element_size() if q is not None else 8, KF._ptr(qrows), u.numel(),
+                KF._ptr(cat), cat.stride(0), cat.shape[0], id_base, KF._ptr(gptr), KF._ptr(gids))
+        if gold_scores is None:
+            gold_scores = torch.zeros(n_gold, dtype=torch.float32, device=dev)
+            _lib.check(lib.kgrec_rec_gold_scores(*head, KF._ptr(gumbel_u), seed, KF._ptr(gold_scores), KF._stream()))
+            KF.count_launches(1)
+        return (lib, head, gumbel_u, seed, gold_scores, (q, qrows, cat)), n_gold, dev     # head holds raw pointers into the last
+
+    def gold_scores_items(self, u_ids, gold_csr, catalog=None, id_base=0, soft_catalog=None, gumbel_u=None, seed=0, topn=0,
+                          n_gold=None):
+        """float32 [n_gold]: score(user, gold) of every gold of gold_csr that lies in the catalog shard, 0 elsewhere,
+        computed by the sweep rank_counts_items compares against.  Arrays of different shards add (one all-reduce);
+        pass the sum as rank_counts_items(gold_scores=...) on every shard, with the same user list and seed."""
+        call, n_gold, dev = self._rank_call(u_ids, gold_csr, None, catalog, id_base, soft_catalog, gumbel_u, seed, topn, n_gold, None)
+        return call[4] if call else torch.zeros(n_gold, dtype=torch.float32, device=dev)
+
+    def rank_counts_items(self, u_ids, gold_csr, filter_csr=None, catalog=None, id_base=0, soft_catalog=None, gumbel_u=None,
+                          seed=None, gold_scores=None, topn=0, n_gold=None):
+        """int32 [n_gold]: for every gold item of every user (gold_csr = (int64 ptr [n_users + 1], int32 ascending
+        ids)), the number of catalog items ranked before it in the (score, id) order of topk_items, leaving out the
+        user's filter row (filter_csr, as topk_items takes it) and the user's other golds; -1 for a gold that is itself
+        filtered (kgrec_rec_rank_count).  One query per user: with hashed ST-Gumbel noise the scores are those
+        topk_items sees for the same user list and seed.  topn selects the path topk_items(k=topn) takes.
+        catalog / id_base / soft_catalog: a shard, as in topk_items; per-shard counts add (sharded_rank_counts; a
+        skipped gold is then negative) once gold_scores holds the summed gold_scores_items of all shards."""
+        call, n_gold, dev = self._rank_call(u_ids, gold_csr, filter_csr, catalog, id_base, soft_catalog, gumbel_u, seed, topn,
+                                            n_gold, gold_scores)
+        counts = torch.zeros(n_gold, dtype=torch.int32, device=dev)
+        if call:
+            lib, head, gumbel_u, seed, gs, _alive = call
+            fptr, fids = filter_csr if filter_csr is not None else (None, None)
+            ws = torch.empty(int(lib.kgrec_rec_rank_workspace_bytes(head[5], n_gold)) // 8 + 1, dtype=torch.int64, device=dev)
+            _lib.check(lib.kgrec_rec_rank_count(*head, n_gold, KF._ptr(gs.contiguous().float()), KF._ptr(fptr), KF._ptr(fids),
+                                                KF._ptr(gumbel_u), seed, KF._ptr(counts), KF._ptr(ws), ws.numel() * 8, KF._stream()))
+            KF.count_launches(3)      # gold sort, catalog sweep, prefix sums
+        return counts
+
     def rank_loss(self, pos, neg, target=-1.0, loss="bpr", batch_pos=None, gumbel_u=None):
         """Fused pos + K negatives + ranking loss: pos = (u, i), neg = (u repeated, ni)."""
         pos = (pos[0], pos[1], None)
