@@ -1877,12 +1877,14 @@ extern "C" int kgrec_corrupt_loss_step(const kgrec_tables* tables, int model, co
     set_error("TransR step kernel: embedding_size <= 128 and at most 14 negatives per positive");
     return KGREC_ERR_UNSUPPORTED;
   }
-  if (n_pos == 0) return KGREC_OK;
+  // checked before the n_pos == 0 return, so that an empty call accepts exactly the shapes a real one does (at
+  // n_pos = 0 the 32-bit products of group_on_registers hold and the rule reduces to d <= 128, at most 32 negatives)
   const bool on_registers = group_on_registers(pl, tables, n_pos, n_neg);
   if (reg_flags && pl.fam != FAM_R && !on_registers) {
     set_error("fused regularisers are built for the d <= 128 margin-loss step kernels only");
     return KGREC_ERR_UNSUPPORTED;
   }
+  if (n_pos == 0) return KGREC_OK;
   const GroupArgs G = group_args(tables, ph, pt, pr, idx_bytes, n_pos, corrupt, n_neg, batch_pos, loss_kind, margin_or_target,
                                  pl.fam != FAM_R);
   float* group_loss = static_cast<float*>(workspace);
