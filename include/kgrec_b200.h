@@ -282,7 +282,9 @@ typedef struct kgrec_opt_table {
   const int32_t* marks;  /* [rows] epoch marks, or NULL = all rows                             */
   int64_t rows;
   int32_t dim;
-  int32_t keep_acc;      /* 1: leave acc as it is (another table entry shares it and clears it) */
+  int32_t keep_acc;      /* 1: leave acc as it is (an entry of a LATER call shares it and clears  */
+                         /* it).  An update call refuses entries whose accumulators overlap when  */
+                         /* one of them clears its own: the other could read it already cleared   */
   int32_t vec;           /* set by the library (128-bit path usable)                           */
   int32_t reserved;
 } kgrec_opt_table;
@@ -299,8 +301,10 @@ typedef struct kgrec_mark_seg {
   int64_t rows;
 } kgrec_mark_seg;
 
-/* marks[id] = epoch for every id of every segment (<= 8 segments, one launch).  Out-of-range ids
- * are skipped and reported through status (optional int32[1]). */
+/* marks[id] = epoch for every id of every segment (<= 8 segments, one launch).  An id is first
+ * decoded (compact: v < 0 names ~v), then remapped, then range-checked.  An out-of-range id (of the
+ * remap, or of the table) marks row 0 -- where the training kernels clamp it and send its gradient --
+ * and sets *status (optional int32[1]) to 1; a call with every id in range leaves *status as it is. */
 int kgrec_rows_mark(const kgrec_mark_seg* segs_host, int n_segs, int32_t epoch, int32_t* status,
                     kgrec_stream_t stream);
 /* adds to *sqnorm the squared L2 norm of the marked accumulator rows of all tables:

@@ -371,6 +371,22 @@ static int sweep_args(const kgrec_opt_table* tabs, int n_tabs, int32_t epoch, in
     A.chunk_begin[t + 1] = A.chunk_begin[n_tabs];
     A.unit_begin[t + 1] = A.unit_begin[n_tabs];
   }
+  // An update clears an entry's accumulator rows as it consumes them, and the warps of all the entries of a call run
+  // concurrently: another entry of the same call reading that memory could see it cleared already.  keep_acc = 1
+  // shares an accumulator with an entry of a later call only.
+  if (need_table)
+    for (int t = 0; t < n_tabs; ++t)
+      for (int o = 0; o < n_tabs; ++o) {
+        if (o == t || tabs[o].keep_acc) continue;
+        const uintptr_t t0 = reinterpret_cast<uintptr_t>(tabs[t].acc), o0 = reinterpret_cast<uintptr_t>(tabs[o].acc);
+        const uintptr_t t1 = t0 + static_cast<uintptr_t>(tabs[t].rows) * tabs[t].dim * sizeof(float);
+        const uintptr_t o1 = o0 + static_cast<uintptr_t>(tabs[o].rows) * tabs[o].dim * sizeof(float);
+        if (t0 < o1 && o0 < t1) {
+          set_error("sparse row optimizer: table %d reads the accumulator that table %d of the same call clears "
+                    "(keep_acc = 0); an accumulator cleared by one entry is read by no other entry of the call", t, o);
+          return KGREC_ERR_INVALID;
+        }
+      }
   return KGREC_OK;
 }
 
