@@ -527,6 +527,26 @@ int kgrec_eval_rank_count_ex(const kgrec_tables* tables, int model, int side,
                              const int32_t* excl_row, const int64_t* excl_ptr, const int32_t* excl_ids,
                              kgrec_stream_t stream);
 
+/* Raw and filtered ranks of link prediction from one catalog sweep.  The arguments of kgrec_eval_rank_count_ex
+ * (counts -> filt_counts: the same count, bit for bit) plus the query's gold set as a CSR indexed by the same row,
+ * G_i = gold_set_ids[gold_ptr[excl_row[i]], gold_ptr[excl_row[i] + 1]) (ascending global ids), and raw_counts:
+ *
+ *   filt_counts[i] += #{ e in shard : (score(q_i, e), e) < (gold_scores[i], gold_ids[i]), e not in X_i }
+ *   raw_counts[i]  += #{ e in shard : (score(q_i, e), e) < (gold_scores[i], gold_ids[i]), e not in G_i }
+ *
+ * raw is the reference's walk without the filter (fliter_samples = None, utils/misc.py:125-146): only the query's
+ * other golds are skipped.  PRECONDITION: every id of G_i is also in X_i (X_i = filter set U gold set, as
+ * KGEvaluator builds it); the gold row is searched only for ids the exclusion row holds, so a gold missing from X_i
+ * counts in the raw count.  Both arrays caller-zeroed; the counts of catalog shards add.  KG sides only; every
+ * array non-NULL and aligned to its element size. */
+int kgrec_eval_rank_count_dual(const kgrec_tables* tables, int model, int side,
+                               const void* q, const void* r, int idx_bytes, const float* qvec, int64_t nq,
+                               const float* cat, int64_t cat_ld, int64_t n_cat, int64_t id_base,
+                               const float* gold_scores, const int32_t* gold_ids, int32_t* filt_counts,
+                               const int32_t* excl_row, const int64_t* excl_ptr, const int32_t* excl_ids,
+                               const int64_t* gold_ptr, const int32_t* gold_set_ids, int32_t* raw_counts,
+                               kgrec_stream_t stream);
+
 /* Rank counts of the recommendation side (TUP / KTUP): where every gold item of a user sits in the whole filtered
  * catalog.  The queries are USERS, one query per user exactly as in kgrec_eval_topk on KGREC_SIDE_REC (q = user ids,
  * or qvec = augmented user rows with cat = the augmented catalog of the same kind: kgrec_pref_aug_rows /
@@ -603,6 +623,15 @@ int kgrec_transr_eval_rank_count_ex(const kgrec_tables* tables, int side, const 
                                     const float* gold_scores, const int32_t* gold_ids, int32_t* counts,
                                     const int32_t* excl_row, const int64_t* excl_ptr, const int32_t* excl_ids,
                                     int32_t* status, kgrec_stream_t stream);
+/* kgrec_eval_rank_count_dual on the projected rows: excl_row (sorted query order) indexes both CSRs with
+ * absolute rows; filt_counts / raw_counts are in the sorted query order. */
+int kgrec_transr_eval_rank_count_dual(const kgrec_tables* tables, int side, const void* q, const void* r, int idx_bytes,
+                                      int64_t nq, const int64_t* run_begin_host, const int64_t* run_rel_host, int32_t n_runs,
+                                      const float* cat, int64_t cat_ld, int64_t n_cat, int64_t id_base, float* workspace,
+                                      const float* gold_scores, const int32_t* gold_ids, int32_t* filt_counts,
+                                      const int32_t* excl_row, const int64_t* excl_ptr, const int32_t* excl_ids,
+                                      const int64_t* gold_ptr, const int32_t* gold_set_ids, int32_t* raw_counts,
+                                      int32_t* status, kgrec_stream_t stream);
 
 /* Soft-preference rec-side evaluation (use_st_gumbel = 0) on augmented rows: with raw logits as
  * mixing weights (transUP.py:108-113) r and w are linear in the logits, so each table row is

@@ -603,16 +603,21 @@ __device__ __noinline__ uint32_t topk_insert_candidates(unsigned mask, uint32_t 
 constexpr int RQ = 8;                         // queries per warp
 
 struct TiledSmem {
-  size_t bars, q, w, gold, tiles, lists, total, excl;
+  size_t bars, q, w, gold, tiles, lists, total, excl, gexcl;
 };
 
 // Exclusion CSR of the filtered rank count (kgrec_eval_rank_count_ex): row i of the launch skips the global ids
 // ids[ptr[row[i]], ptr[row[i] + 1]) (ascending).  A kernel parameter of its own, behind the existing ones, so the
 // layout of EvalArgs and of the other parameters is that of the unfiltered instantiations.
+// The dual count (kgrec_eval_rank_count_dual) adds the gold CSR, indexed by the same row (gold_ids[gold_ptr[row[i]],
+// gold_ptr[row[i] + 1]), ascending, a subset of the exclusion row), and the raw counts; the other modes leave them NULL.
 struct ExclArgs {
   const int32_t* row;
   const int64_t* ptr;
   const int32_t* ids;
+  const int64_t* gold_ptr;
+  const int32_t* gold_ids;
+  int32_t* raw;
 };
 // Row pitch of a catalog tile in shared memory (floats).  A lane reads one 16-byte chunk of "its" row per step, so
 // 8 consecutive rows must land on 8 different bank groups: true when the row is an odd number of 16-byte units long
@@ -624,7 +629,7 @@ __host__ __device__ inline int tile_pitch(int d) { return ((d >> 2) & 1) ? d : d
 // ST-Gumbel rec rows: [x (d) | A_k = x . P'_k / 2 (P) | C_k = x . W_k (P) | pad to a multiple of 4]
 __host__ __device__ inline int gumbel_aug_ld(int d, int P) { return (d + 2 * P + 3) & ~3; }
 __host__ __device__ inline TiledSmem tiled_smem_layout(int kind, int mode, int d, int tn, int stages, int k, int warps, int P = 0,
-                                                       bool excl = false) {
+                                                       bool excl = false, bool dual = false) {
   TiledSmem s{};
   const int TQT = RQ * warps;
   size_t off = 0;
@@ -640,6 +645,9 @@ __host__ __device__ inline TiledSmem tiled_smem_layout(int kind, int mode, int d
   if (mode == MODE_RANK && excl) {        // per-query exclusion range [lo, hi) of the filtered rank count
     s.excl = off; off += static_cast<size_t>(TQT) * 2 * sizeof(int64_t);
   }
+  if (mode == MODE_RANK && excl && dual) {   // per-query gold range [lo, hi) of the dual count
+    s.gexcl = off; off += static_cast<size_t>(TQT) * 2 * sizeof(int64_t);
+  }
   off = (off + 127) & ~static_cast<size_t>(127);
   s.tiles = off; off += static_cast<size_t>(stages) * tn * tile_pitch(kind == KIND_GUMBEL_L2 ? gumbel_aug_ld(d, P) : d) * sizeof(float);
   if (mode == MODE_TOPK) { s.lists = off; off += static_cast<size_t>(TQT) * k * sizeof(uint64_t); }
@@ -649,10 +657,16 @@ __host__ __device__ inline TiledSmem tiled_smem_layout(int kind, int mode, int d
 
 // EXCL (MODE_RANK only): a row counts only when its key is below the gold key AND its id is not in the query's
 // exclusion row (X); the id is looked up after the key test, so rows ranked behind the gold cost nothing extra.
-template <int KIND, int MODE, bool L1, int RN, int W, bool IDS, bool EXCL = false>
+// DUAL (with EXCL): one sweep keeps the filtered count above and the raw count, which skips only the query's golds:
+// a row below the gold key that is not excluded counts in both; an excluded one counts in the raw count unless the
+// second search, over the gold row (a subset of the exclusion row), finds it.  Rows behind the gold and rows not
+// excluded cost no second search.  Excluded non-gold rows below the gold are few (at most the filter set), so they
+// go to X.raw as single atomics instead of a second register counter per query (which spills the 8 x 4 L2 tile).
+template <int KIND, int MODE, bool L1, int RN, int W, bool IDS, bool EXCL = false, bool DUAL = false>
 __global__ void __launch_bounds__(W * 32, 1)
 k_eval_tiled(const EvalArgs A, const int stages, const int64_t units_per_cta, const ExclArgs X) {
   static_assert(!EXCL || MODE == MODE_RANK, "the exclusion CSR belongs to the rank count");
+  static_assert(!DUAL || EXCL, "the dual count extends the filtered count");
   extern __shared__ __align__(128) unsigned char smem_raw[];
   constexpr int TN = 32 * RN;
   constexpr int TQT = RQ * W;
@@ -660,13 +674,14 @@ k_eval_tiled(const EvalArgs A, const int stages, const int64_t units_per_cta, co
   const kgrec_tables& T = A.T;
   const int d = T.dim;
   const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-  const TiledSmem L = tiled_smem_layout(KIND, MODE, d, TN, stages, A.k, W, T.n_pref, EXCL);
+  const TiledSmem L = tiled_smem_layout(KIND, MODE, d, TN, stages, A.k, W, T.n_pref, EXCL, DUAL);
   uint64_t* full = reinterpret_cast<uint64_t*>(smem_raw + L.bars);
   uint64_t* empty = full + 8;
   float* sQ = reinterpret_cast<float*>(smem_raw + L.q);
   [[maybe_unused]] float* sW = reinterpret_cast<float*>(smem_raw + L.w);
   [[maybe_unused]] uint32_t* sGold = reinterpret_cast<uint32_t*>(smem_raw + L.gold);
   [[maybe_unused]] int64_t* sExcl = reinterpret_cast<int64_t*>(smem_raw + L.excl);
+  [[maybe_unused]] int64_t* sGx = reinterpret_cast<int64_t*>(smem_raw + L.gexcl);
   float* tiles = reinterpret_cast<float*>(smem_raw + L.tiles);
   const int rf = (KIND == KIND_GUMBEL_L2) ? gumbel_aug_ld(d, T.n_pref) : d;   // floats of a catalog row that travel
   const int pitch = tile_pitch(rf);
@@ -719,6 +734,7 @@ k_eval_tiled(const EvalArgs A, const int stages, const int64_t units_per_cta, co
   [[maybe_unused]] const float* wq = sW + wid * RQ * d;
   [[maybe_unused]] const uint32_t* gq = sGold + wid * RQ * 2;
   [[maybe_unused]] const int64_t* xq = sExcl + wid * RQ * 2;
+  [[maybe_unused]] const int64_t* gxq = sGx + wid * RQ * 2;
   const int nk4 = d >> 2;
   // Every row is walked in the same dimension order, so a (query, row) score is bit-identical wherever the row
   // sits (tile, lane, shard, gathered sub-catalog).
@@ -788,6 +804,18 @@ k_eval_tiled(const EvalArgs A, const int stages, const int64_t units_per_cta, co
             sExcl[(wid * RQ + qi) * 2 + 1] = hi;
           }
         }
+        if constexpr (DUAL) {
+          if (lane == 2) {
+            int64_t lo = 0, hi = 0;
+            if (q < A.nq) {
+              const int64_t row = __ldg(X.row + q);
+              lo = __ldg(X.gold_ptr + row);
+              hi = __ldg(X.gold_ptr + row + 1);
+            }
+            sGx[(wid * RQ + qi) * 2] = lo;
+            sGx[(wid * RQ + qi) * 2 + 1] = hi;
+          }
+        }
       }
     }
 #pragma unroll
@@ -815,6 +843,8 @@ k_eval_tiled(const EvalArgs A, const int stages, const int64_t units_per_cta, co
 #pragma unroll
         for (int o = 16; o > 0; o >>= 1) c += __shfl_xor_sync(FULL, c, o);
         if (lane == 0 && q0 + qi < A.nq && c) atomicAdd(A.counts + q0 + qi, c);
+        if constexpr (DUAL)
+          if (lane == 0 && q0 + qi < A.nq && c) atomicAdd(X.raw + q0 + qi, c);
       }
     }
   };
@@ -1005,7 +1035,12 @@ k_eval_tiled(const EvalArgs A, const int stages, const int64_t units_per_cta, co
         } else if constexpr (MODE == MODE_RANK) {
           const uint32_t id = static_cast<uint32_t>(A.id_base + n_local);
           const uint32_t gh = gq[qi * 2], gi = gq[qi * 2 + 1];
-          if constexpr (EXCL) {
+          if constexpr (DUAL) {
+            if (valid && (sb < gh || (sb == gh && id < gi))) {
+              if (!filtered(X.ids, xq[qi * 2], xq[qi * 2 + 1], static_cast<int32_t>(id))) ++cnt[qi];
+              else if (!filtered(X.gold_ids, gxq[qi * 2], gxq[qi * 2 + 1], static_cast<int32_t>(id))) atomicAdd(X.raw + q, 1);
+            }
+          } else if constexpr (EXCL) {
             if (valid && (sb < gh || (sb == gh && id < gi)) && !filtered(X.ids, xq[qi * 2], xq[qi * 2 + 1], static_cast<int32_t>(id)))
               ++cnt[qi];
           } else {
@@ -1424,7 +1459,8 @@ static int eval_rotate() {
 }
 
 static int eval_plan(const kgrec_tables* T, int model, int side, int mode, const float* cat, int64_t cat_ld,
-                     int64_t nq, int64_t n_cat, int k, bool have_qvec, EvalArgs* A, EvalPlan* pl, bool excl = false) {
+                     int64_t nq, int64_t n_cat, int k, bool have_qvec, EvalArgs* A, EvalPlan* pl, bool excl = false,
+                     bool dual = false) {
   if (!T) { set_error("tables is NULL"); return KGREC_ERR_INVALID; }
   if (!cat || n_cat <= 0 || nq <= 0) { set_error("empty catalog / query set"); return KGREC_ERR_INVALID; }
   const int d = T->dim;
@@ -1526,9 +1562,9 @@ static int eval_plan(const kgrec_tables* T, int model, int side, int mode, const
       pl->rn = (pl->kind == KIND_DIST ? 4 : 2) / (warps == 16 ? 1 : 2);
       tn_t = 32 * pl->rn;
       int stages = 4;
-      while (stages > 2 && tiled_smem_layout(pl->kind, mode, d, tn_t, stages, k, warps, 0, excl).total > 210 * 1024) --stages;
+      while (stages > 2 && tiled_smem_layout(pl->kind, mode, d, tn_t, stages, k, warps, 0, excl, dual).total > 210 * 1024) --stages;
       pl->stages = stages;
-      pl->smem = tiled_smem_layout(pl->kind, mode, d, tn_t, stages, k, warps, 0, excl).total;
+      pl->smem = tiled_smem_layout(pl->kind, mode, d, tn_t, stages, k, warps, 0, excl, dual).total;
       if (pl->smem <= 225 * 1024 || warps == 4 || (warps == 8 && mode != MODE_TOPK)) break;
     }
     pl->tn = tn_t;
@@ -1598,6 +1634,7 @@ static int launch_eval(const EvalArgs& A, const EvalPlan& pl, cudaStream_t st, c
     }                                                                                                         \
     if constexpr (MODE == MODE_RANK) {                                                                        \
       if (X.row) kern = A.T.l1 ? k_eval_tiled<KINDV, MODE, true, RNV, WV, false, true> : k_eval_tiled<KINDV, MODE, false, RNV, WV, false, true>; \
+      if (X.raw) kern = A.T.l1 ? k_eval_tiled<KINDV, MODE, true, RNV, WV, false, true, true> : k_eval_tiled<KINDV, MODE, false, RNV, WV, false, true, true>; \
     }                                                                                                         \
     KGREC_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(pl.smem))); \
     kern<<<pl.grid, WV * 32, pl.smem, st>>>(A, pl.stages, pl.units_per_cta, X);                               \
@@ -1832,14 +1869,16 @@ extern "C" int kgrec_merge_topk(const uint64_t* in_keys, int32_t n_lists, int64_
   return KGREC_OK;
 }
 
-// kgrec_eval_rank_count (X == NULL) and kgrec_eval_rank_count_ex (X = the exclusion CSR)
+// kgrec_eval_rank_count (X == NULL), kgrec_eval_rank_count_ex (X = the exclusion CSR) and kgrec_eval_rank_count_dual
+// (X->raw set: the exclusion CSR, the gold CSR and the raw counts)
 static int rank_count(const kgrec_tables* tables, int model, int side, const void* q, const void* r, int idx_bytes,
                       const float* qvec, int64_t nq, const float* cat, int64_t cat_ld, int64_t n_cat, int64_t id_base,
                       const float* gold_scores, const int32_t* gold_ids, int32_t* counts, const ExclArgs* X,
                       kgrec_stream_t stream) {
   EvalArgs A{};
   EvalPlan pl{};
-  int rc = eval_plan(tables, model, side, MODE_RANK, cat, cat_ld, nq, n_cat, 0, qvec != nullptr, &A, &pl, X != nullptr);
+  const bool dual = X && X->raw;
+  int rc = eval_plan(tables, model, side, MODE_RANK, cat, cat_ld, nq, n_cat, 0, qvec != nullptr, &A, &pl, X != nullptr, dual);
   if (rc) return rc;
   if (!gold_scores || !gold_ids || !counts) { set_error("rank_count: NULL argument"); return KGREC_ERR_INVALID; }
   if (!qvec && (!q || (side != KGREC_SIDE_REC && !r))) { set_error("query ids are NULL"); return KGREC_ERR_INVALID; }
@@ -1850,6 +1889,12 @@ static int rank_count(const kgrec_tables* tables, int model, int side, const voi
     if (!X->row || !X->ptr || !X->ids) { set_error("rank_count_ex: exclusion CSR (excl_row / excl_ptr / excl_ids) has a NULL array"); return KGREC_ERR_INVALID; }
     if ((reinterpret_cast<uintptr_t>(X->row) & 3u) || (reinterpret_cast<uintptr_t>(X->ptr) & 7u) || (reinterpret_cast<uintptr_t>(X->ids) & 3u)) {
       set_error("rank_count_ex: exclusion CSR arrays are not aligned to their element size");
+      return KGREC_ERR_INVALID;
+    }
+    if (dual && (!X->gold_ptr || !X->gold_ids)) { set_error("rank_count_dual: gold CSR (gold_ptr / gold_set_ids) has a NULL array"); return KGREC_ERR_INVALID; }
+    if (dual && ((reinterpret_cast<uintptr_t>(X->gold_ptr) & 7u) || (reinterpret_cast<uintptr_t>(X->gold_ids) & 3u) ||
+                 (reinterpret_cast<uintptr_t>(X->raw) & 3u) || (reinterpret_cast<uintptr_t>(counts) & 3u))) {
+      set_error("rank_count_dual: gold CSR / count arrays are not aligned to their element size");
       return KGREC_ERR_INVALID;
     }
     if (!pl.tiled) { set_error("rank_count_ex: filtered rank counts are built for the KG sides"); return KGREC_ERR_UNSUPPORTED; }
@@ -1875,6 +1920,18 @@ extern "C" int kgrec_eval_rank_count_ex(const kgrec_tables* tables, int model, i
                                         const int32_t* excl_ids, kgrec_stream_t stream) {
   const ExclArgs X{excl_row, excl_ptr, excl_ids};
   return rank_count(tables, model, side, q, r, idx_bytes, qvec, nq, cat, cat_ld, n_cat, id_base, gold_scores, gold_ids, counts,
+                    &X, stream);
+}
+
+extern "C" int kgrec_eval_rank_count_dual(const kgrec_tables* tables, int model, int side, const void* q, const void* r,
+                                          int idx_bytes, const float* qvec, int64_t nq, const float* cat, int64_t cat_ld,
+                                          int64_t n_cat, int64_t id_base, const float* gold_scores, const int32_t* gold_ids,
+                                          int32_t* filt_counts, const int32_t* excl_row, const int64_t* excl_ptr,
+                                          const int32_t* excl_ids, const int64_t* gold_ptr, const int32_t* gold_set_ids,
+                                          int32_t* raw_counts, kgrec_stream_t stream) {
+  if (!raw_counts) { set_error("rank_count_dual: NULL argument (raw_counts)"); return KGREC_ERR_INVALID; }
+  const ExclArgs X{excl_row, excl_ptr, excl_ids, gold_ptr, gold_set_ids, raw_counts};
+  return rank_count(tables, model, side, q, r, idx_bytes, qvec, nq, cat, cat_ld, n_cat, id_base, gold_scores, gold_ids, filt_counts,
                     &X, stream);
 }
 

@@ -285,3 +285,32 @@ extern "C" int kgrec_transr_eval_rank_count_ex(const kgrec_tables* tables, int s
   return KGREC_OK;
 }
 
+extern "C" int kgrec_transr_eval_rank_count_dual(const kgrec_tables* tables, int side, const void* q, const void* r, int idx_bytes,
+                                                 int64_t nq, const int64_t* run_begin_host, const int64_t* run_rel_host, int32_t n_runs,
+                                                 const float* cat, int64_t cat_ld, int64_t n_cat, int64_t id_base, float* workspace,
+                                                 const float* gold_scores, const int32_t* gold_ids, int32_t* filt_counts,
+                                                 const int32_t* excl_row, const int64_t* excl_ptr, const int32_t* excl_ids,
+                                                 const int64_t* gold_ptr, const int32_t* gold_set_ids, int32_t* raw_counts,
+                                                 int32_t* status, kgrec_stream_t stream) {
+  TRANSR_CALL();
+  if (!gold_scores || !gold_ids || !filt_counts || !raw_counts) { set_error("rank_count_dual: NULL argument"); return KGREC_ERR_INVALID; }
+  if (!excl_row || !excl_ptr || !excl_ids) { set_error("rank_count_ex: exclusion CSR (excl_row / excl_ptr / excl_ids) has a NULL array"); return KGREC_ERR_INVALID; }
+  if (!gold_ptr || !gold_set_ids) { set_error("rank_count_dual: gold CSR (gold_ptr / gold_set_ids) has a NULL array"); return KGREC_ERR_INVALID; }
+  if ((reinterpret_cast<uintptr_t>(excl_row) & 3u) || (reinterpret_cast<uintptr_t>(excl_ptr) & 7u) || (reinterpret_cast<uintptr_t>(excl_ids) & 3u) ||
+      (reinterpret_cast<uintptr_t>(gold_ptr) & 7u) || (reinterpret_cast<uintptr_t>(gold_set_ids) & 3u) ||
+      (reinterpret_cast<uintptr_t>(filt_counts) & 3u) || (reinterpret_cast<uintptr_t>(raw_counts) & 3u)) {
+    set_error("rank_count_dual: exclusion / gold CSR or count arrays are not aligned to their element size");
+    return KGREC_ERR_INVALID;
+  }
+  if (id_base < 0 || id_base + n_cat > 0xffffffffll) { set_error("catalog ids must fit 32 bits"); return KGREC_ERR_INVALID; }
+  const int d = tables->dim;
+  for (int g = 0; g < n_runs; ++g) {
+    if ((rc = transr_prepare(C, g))) return rc;
+    const int64_t i0 = run_begin_host[g], n = run_begin_host[g + 1] - i0;
+    rc = kgrec_eval_rank_count_dual(tables, KGREC_TRANSR, side, nullptr, nullptr, 8, C.qvec_ws + i0 * 2 * d, n, C.proj_ws, d, n_cat,
+                                    id_base, gold_scores + i0, gold_ids + i0, filt_counts + i0, excl_row + i0, excl_ptr, excl_ids,
+                                    gold_ptr, gold_set_ids, raw_counts + i0, stream);
+    if (rc) return rc;
+  }
+  return KGREC_OK;
+}

@@ -163,6 +163,10 @@ _SIGNATURES = {
                                            C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_int64, C.c_int64,
                                            C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                            C.c_void_p]),
+    "kgrec_eval_rank_count_dual": (C.c_int, [C.POINTER(Tables), C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int,
+                                             C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_int64, C.c_int64,
+                                             C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                             C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "kgrec_rec_topk_metrics": (C.c_int, [C.c_void_p, C.c_int64, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
                                          C.c_void_p]),
     "kgrec_rec_gold_scores": (C.c_int, [C.POINTER(Tables), C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_int64, C.c_void_p,
@@ -188,6 +192,11 @@ _SIGNATURES = {
                                                   C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_int64, C.c_int64,
                                                   C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                                   C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "kgrec_transr_eval_rank_count_dual": (C.c_int, [C.POINTER(Tables), C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_int64,
+                                                    C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_int64, C.c_int64,
+                                                    C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                                    C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                                    C.c_void_p]),
     "kgrec_gumbel_aug_ld": (C.c_int32, [C.c_int32, C.c_int32]),
     "kgrec_gumbel_aug_supported": (C.c_int32, [C.c_int32, C.c_int32, C.c_int32]),
     "kgrec_gumbel_aug_rows": (C.c_int, [C.POINTER(Tables), C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_int64, C.c_int64,

@@ -111,6 +111,63 @@ def csr_from_dicts(keys, dicts, device="cpu", id_lo=0, id_hi=None):
     return torch.from_numpy(ptr).to(device), torch.from_numpy(ids).to(device)
 
 
+# ---- relation categories of link prediction (1-1 / 1-N / N-1 / N-N) ------------------------------------------
+REL_CATEGORIES = ("1-1", "1-N", "N-1", "N-N")
+_REL_TYPE_LABELS = {"one2one": 0, "one2many": 1, "many2one": 2, "many2many": 3}
+
+
+def relation_categories(triples, n_rel):
+    """int8 [n_rel]: the category of every relation, 0 = 1-1, 1 = 1-N, 2 = N-1, 3 = N-N, -1 = absent from `triples`.
+
+    splitRelationType (preprocessTriples.py:14-56) restated on an [n, 3] (h, t, r) array; the reference passes
+    train + valid + test (preprocessTriples.py:253).  avg_head = round(mean over the (t, r) keys of r of |heads|),
+    avg_tail likewise over the (h, r) keys, with Python 3's round (half to even, as np.rint); a relation is N-N when
+    both are > 1, N-1 when only avg_head is, 1-N when only avg_tail is, 1-1 otherwise."""
+    a = np.asarray(triples, dtype=np.int64).reshape(-1, 3)
+    out = np.full(n_rel, -1, dtype=np.int8)
+    if not a.size:
+        return out
+    if a[:, 2].min() < 0 or a[:, 2].max() >= n_rel:
+        raise IndexError("kgrec_b200: a relation id of the triples is outside [0, n_rel)")
+    trip = np.unique(a, axis=0)                        # |heads| of (t, r) counts distinct h, as the reference's sets do
+
+    def avg(key_a, key_b):
+        keys, n_per_key = np.unique(np.stack([key_a, key_b], 1), axis=0, return_counts=True)
+        rel = keys[:, 1]
+        s = np.bincount(rel, weights=n_per_key, minlength=n_rel)
+        k = np.bincount(rel, minlength=n_rel)
+        return np.rint(s / np.maximum(k, 1)), k > 0
+    h, t, r = trip[:, 0], trip[:, 1], trip[:, 2]
+    avg_head, present = avg(t, r)
+    avg_tail, _ = avg(h, r)
+    many_h, many_t = avg_head > 1, avg_tail > 1
+    cat = np.where(many_h, np.where(many_t, 3, 2), np.where(many_t, 1, 0))
+    out[present] = cat[present]
+    return out
+
+
+def load_relation_types(path, n_rel=None):
+    """The reference's `relation_type.dat` (lines `one2one|one2many|many2one|many2many \\t r \\t r ...`, written by
+    preprocessTriples.py:280-284) as the int8 array relation_categories returns, read by each line's label.  n_rel
+    defaults to 1 + the largest relation id in the file.  (The reference's own loadRelationType assigns lines by
+    their position among the non-empty ones, so an empty category shifts the later ones: SURVEY appendix B.)"""
+    rel = {}
+    with open(path, "r", encoding="utf-8") as fin:
+        for line in fin:
+            parts = line.strip().split("\t")
+            if not parts[0]:
+                continue
+            if parts[0] not in _REL_TYPE_LABELS:
+                raise ValueError("kgrec_b200: unknown relation type label %r in %s" % (parts[0], path))
+            for x in parts[1:]:
+                rel[int(x)] = _REL_TYPE_LABELS[parts[0]]
+    n = n_rel if n_rel is not None else 1 + max(rel, default=-1)
+    out = np.full(n, -1, dtype=np.int8)
+    for r, c in rel.items():
+        out[r] = c
+    return out
+
+
 def save_checkpoint(path, model, optimizer=None, step=0, best_step=0, best_dev_performance=0.0):
     """The reference's checkpoint dict (utils/trainer.py:115-122), tensors on the CPU."""
     sd = {k: v.detach().cpu() for k, v in model.state_dict().items()}

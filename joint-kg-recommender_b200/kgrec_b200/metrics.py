@@ -25,6 +25,7 @@ import numpy as np
 import torch
 
 from . import _lib
+from . import dataio as KD
 from . import evaluation as KE
 from . import functional as KF
 
@@ -194,15 +195,41 @@ def _dev_ids(a, dev, dtype):
     return torch.as_tensor(a if a.size else np.zeros(1, a.dtype), device=dev).to(dtype).contiguous()
 
 
+def link_side_arrays(keys, eval_dict, all_dicts, rel_category=None):
+    """side_arrays(..., drop_filtered_gold=False) -- every (query, gold) pair, the filter, exclusion and gold CSRs --
+    plus, per pair:
+      has_filt  bool: the gold is not in its query's filter set, so it has a filtered rank (these are the pairs
+                side_arrays keeps with drop_filtered_gold=True, in the same order)
+      pair_cat  int8 category of the query's relation (rel_category given); a key of eval_dict whose relation has
+                no category (-1, or beyond rel_category) raises ValueError
+    Keys are (entity, relation) tuples."""
+    a = side_arrays(keys, eval_dict, all_dicts, drop_filtered_gold=False)
+    width = 1 + int(max(a["pair_gold"].max(initial=0), a["filt_ids"].max(initial=0)))
+    f_q = np.repeat(np.arange(len(keys), dtype=np.int64), np.diff(a["filt_ptr"]))
+    a["has_filt"] = ~np.isin(a["pair_q"] * width + a["pair_gold"], f_q * width + a["filt_ids"])
+    if rel_category is not None:
+        cat = np.asarray(rel_category)
+        rels = np.fromiter((k[1] for k in eval_dict), dtype=np.int64, count=len(eval_dict))
+        if rels.size and (rels.min() < 0 or rels.max() >= cat.size or (cat[rels] < 0).any()):
+            raise ValueError("kgrec_b200: a relation of the eval dict has no category in rel_category")
+        kr = np.fromiter((k[1] for k in keys), dtype=np.int64, count=len(keys))
+        a["pair_cat"] = cat[kr[a["pair_q"]]].astype(np.int8)
+    return a
+
+
 class _KGSide:
     """Device arrays of one KG side.  TransR keeps its pairs sorted by relation (kgrec_transr_eval_* take the queries
-    of one relation as one run) and maps the ranks back to the driver's order with `inv`."""
+    of one relation as one run) and maps the ranks back to the driver's order with `inv`.
 
-    def __init__(self, model, side, eval_dict, all_dicts, chunk, transr):
+    link=True keeps every (query, gold) pair, `has_filt` (link_side_arrays), the gold CSR and, with rel_category,
+    the per-pair group masks `grp` [1 + 4, n] (row 0: all pairs; row 1 + c: pairs of category c)."""
+
+    def __init__(self, model, side, eval_dict, all_dicts, chunk, transr, link=False, rel_category=None):
         dev = model.device
         self.sd = _lib.SIDE_HEAD if side == "head" else _lib.SIDE_TAIL
         keys = [k for k, gold in eval_dict.items() if len(gold) > 0]
-        a = side_arrays(keys, eval_dict, all_dicts, drop_filtered_gold=True)
+        a = link_side_arrays(keys, eval_dict, all_dicts, rel_category) if link else \
+            side_arrays(keys, eval_dict, all_dicts, drop_filtered_gold=True)
         kq = np.fromiter((k[0] for k in keys), dtype=np.int64, count=len(keys))
         kr = np.fromiter((k[1] for k in keys), dtype=np.int64, count=len(keys))
         q, r, gold, row = kq[a["pair_q"]], kr[a["pair_q"]], a["pair_gold"], a["pair_q"]
@@ -211,6 +238,17 @@ class _KGSide:
             if ids.size and (ids.min() < 0 or ids.max() >= bound):
                 raise IndexError("kgrec_b200: a %s id of the %s eval dict is out of range for its table" % (name, side))
         self.n = int(q.size)
+        if link:
+            self.n_filt = int(a["has_filt"].sum())
+            self.has_filt = torch.as_tensor(a["has_filt"], device=dev)
+            self.kept = torch.as_tensor(np.flatnonzero(a["has_filt"]), device=dev)
+            self.gold_ptr = torch.as_tensor(a["gold_ptr"], device=dev)
+            self.gold_ids = _dev_ids(a["gold_ids"], dev, torch.int32)
+            grp = [np.ones(self.n, dtype=bool)]
+            if rel_category is not None:
+                grp += [a["pair_cat"] == c for c in range(4)]
+            self.grp = torch.as_tensor(np.stack(grp), device=dev)                        # [groups, n] (driver order)
+            self.grp_filt = self.grp & self.has_filt[None, :]
         self.inv = None
         if transr and self.n:
             order = np.argsort(r, kind="stable")
@@ -237,6 +275,9 @@ class _KGSide:
         self.pairs = (kq[a["pair_q"]], kr[a["pair_q"]], a["pair_gold"])    # host copy, driver order
 
 
+LINK_FIELDS = ("n", "rank_sum", "rr_sum", "hits@1", "hits@3", "hits@10", "hits@topn")
+
+
 class KGEvaluator:
     """Filtered KG validation (hit@topn and mean rank of both sides, as evaluate_kg) with the host work done once.
 
@@ -249,17 +290,37 @@ class KGEvaluator:
       3. hit and rank sums as a [4] float64 device tensor.
     result(m) reads it back (the one synchronisation) and returns evaluate_kg's tuple.
     Models: TransE, TransH, TransR, and jTransUP's KG branch (TransH kernels on the KTUP tables, padding row included).
+
+    link=True adds the link-prediction metrics of both settings from the same single sweep per side
+    (kgrec_eval_rank_count_dual / kgrec_transr_eval_rank_count_dual).  For a query q (a key of the eval dict) with
+    gold set G_q and filter set F_q (the union of all_dicts[k][q]), and a gold g of G_q, in (score, id) order:
+      raw(q, g)  = #{ e in catalog : e not in G_q, (s(q, e), e) < (s(q, g), g) }   (the reference's walk without the
+                   filter, -nofilter_wrong_corrupted); every gold has one
+      filt(q, g) = #{ e in catalog : e not in F_q U G_q, (s(q, e), e) < (s(q, g), g) }   (the rank above); a gold
+                   inside F_q has none (-1 in dual_ranks) and is left out of the filtered numbers
+    Ranks are 0-based: MR = mean rank, MRR = mean 1 / (rank + 1), Hits@k = share of pairs with rank < k, for
+    k in (1, 3, 10, topn).  Head and tail are reported apart and combined weighted by their pair counts.  With
+    rel_category (int8 [n_rel], dataio.relation_categories / load_relation_types) every pair is also counted in the
+    category of its relation (1-1 / 1-N / N-1 / N-N), so the categories partition the pairs; a relation of the eval
+    dicts without a category raises.  run() then returns the float64 sums [setting (raw, filtered), side (head, tail),
+    group (all, then the four categories when given), field (LINK_FIELDS)]; link_result(m) turns them into metrics
+    and result(m) still returns evaluate_kg's tuple (the filtered numbers), bit for bit.
     """
 
-    def __init__(self, model, eval_head_dict, eval_tail_dict, all_head_dicts=None, all_tail_dicts=None, topn=10, chunk=512):
+    def __init__(self, model, eval_head_dict, eval_tail_dict, all_head_dicts=None, all_tail_dicts=None, topn=10, chunk=512,
+                 link=False, rel_category=None):
         self.model = model
         self.topn = int(topn)
         self.chunk = int(chunk)
+        self.link = bool(link)
+        if rel_category is not None and not self.link:
+            raise ValueError("kgrec_b200: rel_category needs link=True")
+        self.groups = ("all",) + (tuple(KD.REL_CATEGORIES) if rel_category is not None else ())
         dev = model._require_cuda()
         self._transr = model.MODEL == _lib.TRANSR
         self._kg = _lib.TRANSH if model.MODEL == _lib.KTUP else model.MODEL
-        self.sides = (_KGSide(model, "head", eval_head_dict, all_head_dicts, self.chunk, self._transr),
-                      _KGSide(model, "tail", eval_tail_dict, all_tail_dicts, self.chunk, self._transr))
+        self.sides = (_KGSide(model, "head", eval_head_dict, all_head_dicts, self.chunk, self._transr, self.link, rel_category),
+                      _KGSide(model, "tail", eval_tail_dict, all_tail_dicts, self.chunk, self._transr, self.link, rel_category))
         n_cat, d = model.ent_embeddings.weight.shape
         n_max = max(s.n for s in self.sides)
         c = min(self.chunk, max(1, n_max))
@@ -301,7 +362,10 @@ class KGEvaluator:
 
     def ranks(self):
         """Filtered rank of every (query, gold) pair of the head and the tail side under the current tables: two
-        int32 device tensors in the order evaluate_kg visits the pairs (`sides[i].pairs` holds them on the host)."""
+        int32 device tensors in the order evaluate_kg visits the pairs (`sides[i].pairs` holds them on the host;
+        with link=True, the pairs of `has_filt`)."""
+        if self.link:
+            return tuple(filt.index_select(0, s.kept) for s, (_, filt) in zip(self.sides, self._dual_counts()))
         m = self.model
         dev = m._require_cuda()
         lib = _lib.load()
@@ -329,19 +393,98 @@ class KGEvaluator:
             out.append(counts)
         return tuple(out)
 
+    def _dual_counts(self):
+        """link=True: (raw, filtered) int32 counts of every pair per side, driver order, from one dual sweep per side
+        (a filtered count of a gold inside its filter set is computed but means nothing)."""
+        m = self.model
+        dev = m._require_cuda()
+        lib = _lib.load()
+        T = self._tables()
+        catalog = m.ent_embeddings.weight.detach()
+        n_cat = catalog.shape[0]
+        out = []
+        for s in self.sides:
+            raw = torch.zeros(s.n, dtype=torch.int32, device=dev)
+            filt = torch.zeros(s.n, dtype=torch.int32, device=dev)
+            if s.n:
+                gs = self._gold_scores(T, s, catalog)
+                if self._transr:
+                    _lib.check(lib.kgrec_transr_eval_rank_count_dual(
+                        C.byref(T), s.sd, KF._ptr(s.q), KF._ptr(s.r), 8, s.n, C.c_void_p(s.run_begin.data_ptr()),
+                        C.c_void_p(s.run_rel.data_ptr()), s.run_rel.numel(), KF._ptr(catalog), catalog.stride(0), n_cat, 0,
+                        KF._ptr(self._ws), KF._ptr(gs), KF._ptr(s.gold32), KF._ptr(filt), KF._ptr(s.excl_row),
+                        KF._ptr(s.excl_ptr), KF._ptr(s.excl_ids), KF._ptr(s.gold_ptr), KF._ptr(s.gold_ids), KF._ptr(raw),
+                        KF._ptr(m._status_buf(dev)), KF._stream()))
+                    raw, filt = raw.index_select(0, s.inv), filt.index_select(0, s.inv)
+                else:
+                    _lib.check(lib.kgrec_eval_rank_count_dual(
+                        C.byref(T), self._kg, s.sd, KF._ptr(s.q), KF._ptr(s.r), 8, None, s.n, KF._ptr(catalog),
+                        catalog.stride(0), n_cat, 0, KF._ptr(gs), KF._ptr(s.gold32), KF._ptr(filt), KF._ptr(s.excl_row),
+                        KF._ptr(s.excl_ptr), KF._ptr(s.excl_ids), KF._ptr(s.gold_ptr), KF._ptr(s.gold_ids), KF._ptr(raw),
+                        KF._stream()))
+                    KF.count_launches(1)
+            out.append((raw, filt))
+        return out
+
+    def dual_ranks(self):
+        """link=True: ((head raw, head filtered), (tail raw, tail filtered)) int32 device tensors, one entry per
+        (query, gold) pair in the order evaluate_kg visits them (`sides[i].pairs`); a gold inside its query's filter
+        set has filtered rank -1."""
+        if not self.link:
+            raise ValueError("kgrec_b200: dual_ranks needs KGEvaluator(..., link=True)")
+        return tuple((raw, torch.where(s.has_filt, filt, torch.full_like(filt, -1)))
+                     for s, (raw, filt) in zip(self.sides, self._dual_counts()))
+
+    def _link_sums(self, c, w):
+        """[groups, fields] float64 sums of LINK_FIELDS over the pairs of each group (w: bool [groups, n]).  A plain
+        reduction over a fixed shape, no atomics: the reciprocal-rank sums repeat bit for bit."""
+        c = c.to(torch.float64)
+        vals = torch.stack([torch.ones_like(c), c, 1.0 / (c + 1.0), (c < 1).to(c.dtype), (c < 3).to(c.dtype),
+                            (c < 10).to(c.dtype), (c < self.topn).to(c.dtype)])                  # [fields, n]
+        return torch.where(w[:, None, :], vals[None], torch.zeros((), dtype=c.dtype, device=c.device)).sum(-1)
+
     def run(self):
         """[4] float64 device tensor: (head hits, head rank sum, tail hits, tail rank sum), queued on the current
-        stream with no host synchronisation."""
+        stream with no host synchronisation.  link=True: the [2, 2, groups, 7] sums of the class docstring."""
+        if self.link:
+            per_side = [torch.stack([self._link_sums(raw, s.grp), self._link_sums(filt, s.grp_filt)])
+                        for s, (raw, filt) in zip(self.sides, self._dual_counts())]
+            return torch.stack(per_side, 1)
         parts = []
         for c in self.ranks():
             c = c.to(torch.int64)
             parts += [(c < self.topn).sum(), c.sum()]
         return torch.stack(parts).to(torch.float64)
 
+    def link_result(self, m):
+        """{"raw" | "filtered": {"head" | "tail" | "both": {group: {mr, mrr, hits@1, hits@3, hits@10, hits@topn, n}}}}
+        from the sums run() returned with link=True; "both" pools head and tail pairs; a group without pairs reads 0."""
+        v = m.tolist()
+        out = {}
+        for si, setting in enumerate(("raw", "filtered")):
+            out[setting] = {}
+            for side in ("head", "tail", "both"):
+                out[setting][side] = {}
+                for gi, g in enumerate(self.groups):
+                    if side == "both":
+                        f = [a + b for a, b in zip(v[si][0][gi], v[si][1][gi])]
+                    else:
+                        f = v[si][0 if side == "head" else 1][gi]
+                    n = f[0]
+                    mean = (lambda x: x / n) if n else (lambda x: 0.0)
+                    out[setting][side][g] = {"mr": mean(f[1]), "mrr": mean(f[2]), "hits@1": mean(f[3]), "hits@3": mean(f[4]),
+                                             "hits@10": mean(f[5]), "hits@topn": mean(f[6]), "n": int(n)}
+        return out
+
     def result(self, m):
         """(avg_hit, avg_mean_rank, (head hit, head rank), (tail hit, tail rank)) -- evaluate_kg's tuple, bit for bit."""
-        hh, hr, th, tr = m.tolist()
-        n_h, n_t = self.sides[0].n, self.sides[1].n
+        if self.link:
+            v = m.tolist()
+            hh, hr, th, tr = v[1][0][0][6], v[1][0][0][1], v[1][1][0][6], v[1][1][0][1]
+            n_h, n_t = self.sides[0].n_filt, self.sides[1].n_filt
+        else:
+            hh, hr, th, tr = m.tolist()
+            n_h, n_t = self.sides[0].n, self.sides[1].n
         h = (hh / n_h, hr / n_h) if n_h else (0.0, 0.0)
         t = (th / n_t, tr / n_t) if n_t else (0.0, 0.0)
         tot = max(1, n_h + n_t)
