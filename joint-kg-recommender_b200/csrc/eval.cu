@@ -35,7 +35,10 @@ constexpr int kEvalThreads = kThreads;
 constexpr uint64_t KEY_INF = ~0ull;
 
 // ---- keys -------------------------------------------------------------------------------------
-// scores are sums of |.| or squares: non-negative, so the IEEE bit pattern is monotone
+// Keys order scores by their IEEE bits, which is monotone for non-negative floats only (a set sign bit sorts after
+// +inf).  Every keyed score is non-negative with its sign bit clear: the direct forms are sums of |.| or squares
+// starting from +0, and the one expanded form (KIND_GUMBEL_L2's epilogue in k_eval_tiled) maps -0.0 and negative
+// rounding noise to +0.0.
 __device__ __forceinline__ uint64_t make_key(float s, uint32_t id) {
   return (static_cast<uint64_t>(__float_as_uint(s)) << 32) | id;
 }
@@ -1010,7 +1013,12 @@ k_eval_tiled(const EvalArgs A, const int stages, const int64_t units_per_cta, co
             if (v > best) { best = v; ks = k; }
           }
           const float sd = ua[P + ks] - ia[P + ks];
-          acc[qi][j] += gc[ks] + hf4 * (ua[ks] - ia[ks]) + sd * sd * (gc[P + ks] - 2.f) - 2.f * sd * gc[2 * P + ks];
+          const float v = acc[qi][j] + (gc[ks] + hf4 * (ua[ks] - ia[ks]) + sd * sd * (gc[P + ks] - 2.f) - 2.f * sd * gc[2 * P + ks]);
+          // The expanded form cancels: a pair whose true score is ~0 (a trained positive) comes out as +-rounding
+          // noise.  A set sign bit would key it after every non-negative score, so -0.0 and finite negatives
+          // become +0.0 (within the error bound, the true value being >= 0); -inf and NaN keep their bits.
+          const uint32_t vb = __float_as_uint(v);
+          acc[qi][j] = (vb >= 0x80000000u && vb < 0xff800000u) ? 0.f : v;
         }
       }
     }
